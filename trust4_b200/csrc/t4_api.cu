@@ -42,6 +42,8 @@
 static std::string g_err ;
 static void set_err( const std::string &s ) { g_err = s ; }
 
+#define T4_MIN_BLOCKS 4 // resident CTAs per SM the op kernels are register-bounded for
+
 #if T4_CUDA
 #define CK( call )                                                                 \
 	do                                                                             \
@@ -54,22 +56,12 @@ static void set_err( const std::string &s ) { g_err = s ; }
 		}                                                                          \
 	} while ( 0 )
 
-#ifndef T4_MIN_BLOCKS
-#define T4_MIN_BLOCKS 4
-#endif
+// The kernels are thin wrappers: their bodies are device functions the emulation runs too (see the launchers below).
 __global__ void __launch_bounds__( T4_MAX_NT, T4_MIN_BLOCKS ) t4_stream_kernel( char *A, T4Op *ops, const int *gapTable )
 {
 	__shared__ T4Smem sm ;
-	T4Op *op = ops + blockIdx.x ;
-	T4Ctx cx ;
-	cx.A = A ;
-	cx.g = (T4Global *)A ;
-	cx.st = (T4Stream *)( A + op->streamOff ) ;
-	cx.sm = &sm ;
-	cx.cap = cx.g->cap ;
-	cx.tid = threadIdx.x ;
-	cx.nt = blockDim.x ;
-	c_run_op( cx, op, gapTable ) ;
+	T4Ctx cx = t4_ctx( A, ops[blockIdx.x].streamOff, &sm, threadIdx.x, blockDim.x ) ;
+	c_run_op( cx, ops + blockIdx.x, gapTable ) ;
 }
 
 // The read-only passes over finished sets (t4_assign.h) are a kernel of their own: they share the engine's collectives
@@ -77,16 +69,17 @@ __global__ void __launch_bounds__( T4_MAX_NT, T4_MIN_BLOCKS ) t4_stream_kernel( 
 __global__ void __launch_bounds__( T4_MAX_NT, T4_MIN_BLOCKS ) t4_aux_kernel( char *A, T4Op *ops )
 {
 	__shared__ T4Smem sm ;
-	T4Op *op = ops + blockIdx.x ;
-	T4Ctx cx ;
-	cx.A = A ;
-	cx.g = (T4Global *)A ;
-	cx.st = (T4Stream *)( A + op->streamOff ) ;
-	cx.sm = &sm ;
-	cx.cap = cx.g->cap ;
-	cx.tid = threadIdx.x ;
-	cx.nt = blockDim.x ;
-	c_run_aux_op( cx, op ) ;
+	T4Ctx cx = t4_ctx( A, ops[blockIdx.x].streamOff, &sm, threadIdx.x, blockDim.x ) ;
+	c_run_aux_op( cx, ops + blockIdx.x ) ;
+}
+
+// GetOverlapsFromRead on a reference gene set (t4_annot.h): a kernel of its own, so that the kernels validated on the GPU
+// keep their exact SASS while this one is verified through the emulation only
+__global__ void __launch_bounds__( T4_MAX_NT, T4_MIN_BLOCKS ) t4_annot_kernel( char *A, T4Op *ops )
+{
+	__shared__ T4Smem sm ;
+	T4Ctx cx = t4_ctx( A, ops[blockIdx.x].streamOff, &sm, threadIdx.x, blockDim.x ) ;
+	c_run_annot_op( cx, ops + blockIdx.x ) ;
 }
 
 // one merge pass of the read sort (t4_readsort.h); emulation-verified only, like t4_annot_kernel
@@ -102,21 +95,16 @@ __global__ void t4_mate_overlap_kernel( T4MateParams P )
 		t4_mate_overlap_one( P, i ) ;
 }
 
-// GetOverlapsFromRead on a reference gene set (t4_annot.h): a kernel of its own, so that the kernels validated on the GPU
-// keep their exact SASS while this one is verified through the emulation only
-__global__ void __launch_bounds__( T4_MAX_NT, T4_MIN_BLOCKS ) t4_annot_kernel( char *A, T4Op *ops )
+__global__ void t4_pack_reads_kernel( T4PackReadsParams P )
 {
-	__shared__ T4Smem sm ;
-	T4Op *op = ops + blockIdx.x ;
-	T4Ctx cx ;
-	cx.A = A ;
-	cx.g = (T4Global *)A ;
-	cx.st = (T4Stream *)( A + op->streamOff ) ;
-	cx.sm = &sm ;
-	cx.cap = cx.g->cap ;
-	cx.tid = threadIdx.x ;
-	cx.nt = blockDim.x ;
-	c_run_annot_op( cx, op ) ;
+	for ( i64 g = (i64)blockIdx.x * blockDim.x + threadIdx.x ; g < P.n * P.wMax ; g += (i64)gridDim.x * blockDim.x )
+		t4_pack_read_word( P, g ) ;
+}
+
+__global__ void t4_dp_kernel( T4DpParams P )
+{
+	for ( int i = blockIdx.x * blockDim.x + threadIdx.x ; i < P.n ; i += gridDim.x * blockDim.x )
+		t4_dp_one( P, i ) ;
 }
 
 // k-mer counting / per-read count statistics (t4_kcount.h): persistent warps, batches of reads handed out by an atomic cursor
@@ -135,51 +123,22 @@ __global__ void __launch_bounds__( T4_MAX_NT ) t4_kcount_kernel( T4KcParams P, i
 
 __global__ void t4_init_kernel( char *A, u64 base, T4InitParams ip )
 {
-	__shared__ T4Smem sm ;
-	T4Ctx cx ;
-	cx.A = A ;
-	cx.g = (T4Global *)A ;
-	cx.st = 0 ;
-	cx.sm = &sm ;
-	cx.cap = cx.g->cap ;
-	cx.tid = threadIdx.x ;
-	cx.nt = blockDim.x ;
-	c_init_stream( cx, base + (u64)blockIdx.x * ip.footprint, ip ) ;
+	c_init_block( A, base, ip, blockIdx.x, threadIdx.x, blockDim.x ) ;
 }
 
-// copy contig payloads into one contiguous buffer: per contig [consensus len][posWeight 16*len][name nameLen]
 __global__ void t4_gather_kernel( char *A, const T4Contig *ct, const u64 *outOff, char *out, int n )
 {
-	int c = blockIdx.x ;
-	if ( c >= n || ct[c].consOff == 0 )
-		return ;
-	const T4Contig &k = ct[c] ;
-	char *o = out + outOff[c] ;
-	const char *cons = A + k.consOff + k.lead ;
-	const char *pw = A + k.pwOff + 16ull * k.lead ;
-	const char *nm = A + k.nameOff ;
-	for ( int i = threadIdx.x ; i < k.len ; i += blockDim.x )
-		o[i] = cons[i] ;
-	for ( int i = threadIdx.x ; i < 16 * k.len ; i += blockDim.x )
-		o[k.len + i] = pw[i] ;
-	for ( int i = threadIdx.x ; i < k.nameLen ; i += blockDim.x )
-		o[17 * k.len + i] = nm[i] ;
+	t4_gather_block( A, ct, outOff, out, n, blockIdx.x, threadIdx.x, blockDim.x ) ;
 }
 
-// AlignAlgo::GlobalAlignment_PosWeight for n independent problems, one thread each.
-__global__ void t4_dp_kernel( int n, const int *tw, const i64 *tOff, const char *p, const i64 *pOff, signed char *align,
-	const i64 *alignOff, int *score, char *scratch, const i64 *scratchOff )
+__global__ void t4_pack_size_kernel( char *A, const u64 *streamOff, u64 *sizes, u64 *counts )
 {
-	int i = blockIdx.x * blockDim.x + threadIdx.x ;
-	if ( i >= n )
-		return ;
-	int lent = (int)( tOff[i + 1] - tOff[i] ) ;
-	int lenp = (int)( pOff[i + 1] - pOff[i] ) ;
-	int d = lent > lenp ? lent - lenp : lenp - lent ;
-	int W = 2 * T4_DP_BAND + 3 + d ;
-	char *s = scratch + scratchOff[i] ;
-	score[i] = t4_dp_posweight( tw + 4 * tOff[i], lent, p + pOff[i], lenp, align + alignOff[i], (int *)s,
-		(unsigned char *)( s + 8 * W ), 0 ) ;
+	t4_pack_size_block( A, streamOff, sizes, counts, blockIdx.x, threadIdx.x, blockDim.x ) ;
+}
+
+__global__ void t4_pack_kernel( char *A, const u64 *streamOff, const u64 *outOff, char *out )
+{
+	t4_pack_block( A, streamOff, outOff, out, blockIdx.x, threadIdx.x, blockDim.x ) ;
 }
 
 // Test entry for the two DP routines the stream kernel really runs (equal lengths: overhangs and same-diagonal gaps):
@@ -228,88 +187,6 @@ __global__ void t4_dp_hot_kernel( int n, int variant, const int *tw, const i64 *
 	if ( lane == 0 )
 		score[i] = sc ;
 }
-
-// One CTA per stream: decide for every live contig whether its posWeight counts fit 16 bits (scratch flag in the contig
-// record), and sum the record sizes.
-__global__ void t4_pack_size_kernel( char *A, const u64 *streamOff, u64 *sizes, u64 *counts )
-{
-	const T4Stream *st = (const T4Stream *)( A + streamOff[blockIdx.x] ) ;
-	T4Contig *ct = (T4Contig *)( A + st->seqsOff ) ;
-	u64 tot = 0, n = 0 ;
-	for ( int i = 0 ; i < st->nSeqs ; ++i )
-	{
-		T4Contig &k = ct[i] ;
-		if ( !k.consOff )
-			continue ;
-		const int *pw = (const int *)( A + k.pwOff + 16ull * k.lead ) ;
-		int wide = 0 ;
-		for ( int x = threadIdx.x ; x < 4 * k.len ; x += blockDim.x )
-			wide |= ( (unsigned)pw[x] > 65535u ) ;
-		wide = __syncthreads_or( wide ) ;
-		if ( threadIdx.x == 0 )
-			k.packNarrow = wide ? 0 : 1 ;
-		__syncthreads() ;
-		tot += t4_pack_record_bytes( k ) ;
-		++n ;
-	}
-	if ( threadIdx.x == 0 )
-	{
-		sizes[blockIdx.x] = tot ;
-		counts[blockIdx.x] = n ;
-	}
-}
-
-__global__ void t4_pack_kernel( char *A, const u64 *streamOff, const u64 *outOff, char *out )
-{
-	const T4Stream *st = (const T4Stream *)( A + streamOff[blockIdx.x] ) ;
-	const T4Contig *ct = (const T4Contig *)( A + st->seqsOff ) ;
-	u64 o = outOff[blockIdx.x] ;
-	for ( int i = 0 ; i < st->nSeqs ; ++i )
-	{
-		const T4Contig &k = ct[i] ;
-		if ( !k.consOff )
-			continue ;
-		u64 rb = t4_pack_record_bytes( k ) ;
-		char *rec = out + o ;
-		if ( threadIdx.x == 0 )
-		{
-			u32 *h = (u32 *)rec ;
-			h[0] = blockIdx.x ; h[1] = (u32)i ; h[2] = (u32)k.len ; h[3] = (u32)k.nameLen ;
-			h[4] = (u32)k.barcode ; h[5] = (u32)k.numRead ; h[6] = (u32)rb ; h[7] = k.packNarrow ? 1u : 0u ;
-		}
-		const char *cons = A + k.consOff + k.lead ;
-		const int *pw = (const int *)( A + k.pwOff + 16ull * k.lead ) ;
-		const char *nm = A + k.nameOff ;
-		for ( int x = threadIdx.x ; x < k.len ; x += blockDim.x )
-			rec[32 + x] = cons[x] ;
-		u64 nameAt ;
-		if ( k.packNarrow )
-		{
-			// the columns start at byte 32 + len (any alignment): byte stores
-			unsigned char *d = (unsigned char *)rec + 32 + k.len ;
-			for ( int x = threadIdx.x ; x < 4 * k.len ; x += blockDim.x )
-			{
-				const unsigned v = (unsigned)pw[x] ;
-				d[2 * x] = (unsigned char)( v & 255u ) ;
-				d[2 * x + 1] = (unsigned char)( v >> 8 ) ;
-			}
-			nameAt = 32ull + 9ull * k.len ;
-		}
-		else
-		{
-			const char *pb = (const char *)pw ;
-			for ( int x = threadIdx.x ; x < 16 * k.len ; x += blockDim.x )
-				rec[32 + k.len + x] = pb[x] ;
-			nameAt = 32ull + 17ull * k.len ;
-		}
-		for ( int x = threadIdx.x ; x < k.nameLen ; x += blockDim.x )
-			rec[nameAt + x] = nm[x] ;
-		// tail padding of the 16-byte aligned record: defined bytes (the all-gathered buffers are compared bytewise)
-		for ( u64 x = nameAt + k.nameLen + threadIdx.x ; x < rb ; x += blockDim.x )
-			rec[x] = 0 ;
-		o += rb ;
-	}
-}
 #else
 #define CK( call ) do { } while ( 0 )
 #endif
@@ -318,6 +195,7 @@ struct Engine
 {
 	bool up ;
 	int device ;
+	int sms ;          // SM count of the device
 	char *A ;          // arena base (device or, in the emulation, host)
 	size_t cap ;
 	int nt ;
@@ -329,10 +207,13 @@ struct Engine
 	// grow-only device buffer reused by t4_streams_run for the uploaded workload (no cudaMalloc per call)
 	char *wl ;
 	size_t wlCap ;
-	Engine() : up( false ), device( 0 ), A( 0 ), cap( 0 ), nt( 128 ), gapTable( 0 ), stage( 0 ), stageCap( 0 ), wl( 0 ), wlCap( 0 ) {}
+	Engine() : up( false ), device( 0 ), sms( 0 ), A( 0 ), cap( 0 ), nt( 128 ), gapTable( 0 ), stage( 0 ), stageCap( 0 ), wl( 0 ), wlCap( 0 ) {}
 } ;
 static Engine E ;
 static std::mutex g_mu ;
+
+// workers of the read-only passes (one scratch stream each): one resident wave of the auxiliary kernels
+static int resident_workers() { return T4_CUDA ? E.sms * T4_MIN_BLOCKS : 2 ; }
 
 static int dmalloc( void **p, size_t n )
 {
@@ -362,6 +243,16 @@ static int h2d( void *d, const void *h, size_t n )
 #endif
 	return 0 ;
 }
+// ordered on `stream`; the host buffer may be reused when it returns
+static int h2d_async( void *d, const void *h, size_t n, void *stream )
+{
+#if T4_CUDA
+	CK( cudaMemcpyAsync( d, h, n, cudaMemcpyHostToDevice, (cudaStream_t)stream ) ) ;
+#else
+	memcpy( d, h, n ) ;
+#endif
+	return 0 ;
+}
 static int d2h( void *h, const void *d, size_t n )
 {
 	if ( n == 0 ) return 0 ;
@@ -372,12 +263,126 @@ static int d2h( void *h, const void *d, size_t n )
 #endif
 	return 0 ;
 }
-static int dzero( void *d, size_t n )
+static int dzero( void *d, size_t n, void *stream = 0 )
 {
 #if T4_CUDA
-	CK( cudaMemset( d, 0, n ) ) ;
+	CK( cudaMemsetAsync( d, 0, n, (cudaStream_t)stream ) ) ;
 #else
 	memset( d, 0, n ) ;
+#endif
+	return 0 ;
+}
+static int dsync()
+{
+#if T4_CUDA
+	CK( cudaDeviceSynchronize() ) ;
+#endif
+	return 0 ;
+}
+
+// One device allocation carved into parts in the order they are added, each 256-byte aligned.  add() names the pointer
+// a part goes to; alloc() makes the allocation and sets the pointers (place() sets them into a buffer the caller owns).
+// The allocation is freed when the DevBuf goes out of scope unless keep() hands it over.
+namespace {
+struct DevBuf
+{
+	struct Part { size_t off ; void *ptr ; void ( *set )( void *ptr, char *at ) ; } ;
+	std::vector<Part> parts ;
+	size_t bytes = 0 ;
+	char *base = 0 ;
+	bool owned = false ;
+	template <class T> void add( T *&p, size_t n )
+	{
+		parts.push_back( { bytes, &p, []( void *ptr, char *at ) { *(T **)ptr = (T *)at ; } } ) ;
+		bytes += ( n + 255 ) & ~(size_t)255 ;
+	}
+	void place( char *at )
+	{
+		base = at ;
+		for ( const Part &x : parts )
+			x.set( x.ptr, at + x.off ) ;
+	}
+	int alloc()
+	{
+		void *p = 0 ;
+		int r = dmalloc( &p, bytes ) ;
+		if ( r ) return r ;
+		place( (char *)p ) ;
+		owned = true ;
+		return 0 ;
+	}
+	char *keep() { owned = false ; return base ; }
+	~DevBuf() { if ( owned ) dfree( base ) ; }
+} ;
+}
+
+// ---- launchers: the kernel on the device; in the emulation its device body, in order, on one thread (tid 0, nt 1) ----
+enum { T4K_STREAM, T4K_AUX, T4K_ANNOT } ;
+
+// one CTA of E.nt threads per op record, of the stream, auxiliary or annotation kernel
+static int launch_ops( int kernel, T4Op *dOps, int n, void *stream )
+{
+#if T4_CUDA
+	cudaStream_t cs = (cudaStream_t)stream ;
+	if ( kernel == T4K_STREAM )
+		t4_stream_kernel<<<n, E.nt, 0, cs>>>( E.A, dOps, E.gapTable ) ;
+	else if ( kernel == T4K_AUX )
+		t4_aux_kernel<<<n, E.nt, 0, cs>>>( E.A, dOps ) ;
+	else
+		t4_annot_kernel<<<n, E.nt, 0, cs>>>( E.A, dOps ) ;
+	CK( cudaGetLastError() ) ;
+#else
+	(void)stream ;
+	T4Smem *sm = new T4Smem ;
+	for ( int b = 0 ; b < n ; ++b )
+	{
+		T4Ctx cx = t4_ctx( E.A, dOps[b].streamOff, sm, 0, 1 ) ;
+		if ( kernel == T4K_STREAM )
+			c_run_op( cx, dOps + b, E.gapTable ) ;
+		else if ( kernel == T4K_AUX )
+			c_run_aux_op( cx, dOps + b ) ;
+		else
+			c_run_annot_op( cx, dOps + b ) ;
+	}
+	delete sm ;
+#endif
+	return 0 ;
+}
+
+// The kernel argument of launch_blocks / launch_items: the kernel on the device, its device body in the emulation.
+#if T4_CUDA
+#define T4_KERNEL( kernel, body ) kernel
+#else
+#define T4_KERNEL( kernel, body ) body
+#endif
+
+// grid CTAs of `threads` threads; the emulation runs body( args..., b, 0, 1 ) for every block b
+template <class K, class... A> static int launch_blocks( K kernel, int grid, int threads, A... args )
+{
+#if T4_CUDA
+	kernel<<<grid, threads>>>( args... ) ;
+	CK( cudaGetLastError() ) ;
+#else
+	(void)threads ;
+	for ( int b = 0 ; b < grid ; ++b )
+		kernel( args..., b, 0, 1 ) ;
+#endif
+	return 0 ;
+}
+
+// one thread per item i < n (n > 0), a grid-stride loop over at most 16 CTAs per SM; the emulation runs body( p, i )
+template <class K, class P> static int launch_items( K kernel, const P &p, i64 n, int threads )
+{
+#if T4_CUDA
+	i64 blocks = ( n + threads - 1 ) / threads ;
+	if ( blocks > (i64)E.sms * 16 )
+		blocks = (i64)E.sms * 16 ;
+	kernel<<<(int)blocks, threads>>>( p ) ;
+	CK( cudaGetLastError() ) ;
+#else
+	(void)threads ;
+	for ( i64 i = 0 ; i < n ; ++i )
+		kernel( p, i ) ;
 #endif
 	return 0 ;
 }
@@ -389,62 +394,6 @@ static int nomatch_gap_limit( int kl )
 	double kmerHitProb = pow( readAccuracy, kl ) ;
 	int ret = int( kl * ( log( 0.01 ) / log( 1 - kmerHitProb ) ) ) + 1 ;
 	return ret ;
-}
-
-static int launch_ops( T4Op *dOps, int n, void *stream )
-{
-#if T4_CUDA
-	t4_stream_kernel<<<n, E.nt, 0, (cudaStream_t)stream>>>( E.A, dOps, E.gapTable ) ;
-	CK( cudaGetLastError() ) ;
-#else
-	T4Smem *sm = new T4Smem ;
-	for ( int b = 0 ; b < n ; ++b )
-	{
-		T4Ctx cx ;
-		cx.A = E.A ;
-		cx.g = (T4Global *)E.A ;
-		cx.st = (T4Stream *)( E.A + dOps[b].streamOff ) ;
-		cx.sm = sm ;
-		cx.cap = cx.g->cap ;
-		cx.tid = 0 ;
-		cx.nt = 1 ;
-		c_run_op( cx, dOps + b, E.gapTable ) ;
-	}
-	delete sm ;
-#endif
-	return 0 ;
-}
-
-static int launch_aux_ops( T4Op *dOps, int n, void *stream )
-{
-#if T4_CUDA
-	t4_aux_kernel<<<n, E.nt, 0, (cudaStream_t)stream>>>( E.A, dOps ) ;
-	CK( cudaGetLastError() ) ;
-#else
-	T4Smem *sm = new T4Smem ;
-	for ( int b = 0 ; b < n ; ++b )
-	{
-		T4Ctx cx ;
-		cx.A = E.A ;
-		cx.g = (T4Global *)E.A ;
-		cx.st = (T4Stream *)( E.A + dOps[b].streamOff ) ;
-		cx.sm = sm ;
-		cx.cap = cx.g->cap ;
-		cx.tid = 0 ;
-		cx.nt = 1 ;
-		c_run_aux_op( cx, dOps + b ) ;
-	}
-	delete sm ;
-#endif
-	return 0 ;
-}
-
-static int dsync()
-{
-#if T4_CUDA
-	CK( cudaDeviceSynchronize() ) ;
-#endif
-	return 0 ;
 }
 
 static int ensure_stage( size_t n )
@@ -528,11 +477,7 @@ extern "C" {
 const char *T4_API( last_error )( void ) { return g_err.c_str() ; }
 const char *T4_API( version )( void )
 {
-#if T4_CUDA
-	return "trust4_b200 0.1.0 (sm_90a)" ;
-#else
-	return "trust4_b200 0.1.0 (TEST EMULATION - not a product build)" ;
-#endif
+	return T4_CUDA ? "trust4_b200 0.1.0 (sm_90a)" : "trust4_b200 0.1.0 (TEST EMULATION - not a product build)" ;
 }
 
 int T4_API( shutdown )( void )
@@ -568,6 +513,7 @@ int T4_API( init )( int device, size_t arena_bytes )
 	if ( device < 0 )
 		CK( cudaGetDevice( &device ) ) ;
 	CK( cudaSetDevice( device ) ) ;
+	CK( cudaDeviceGetAttribute( &E.sms, cudaDevAttrMultiProcessorCount, device ) ) ;
 	if ( arena_bytes == 0 )
 	{
 		size_t fr = 0, tot = 0 ;
@@ -675,13 +621,6 @@ int T4_API( last_counters )( uint64_t *c )
 	return 0 ;
 }
 
-static int reset_counters()
-{
-	u64 z[T4_N_COUNTERS] ;
-	memset( z, 0, sizeof( z ) ) ;
-	return h2d( E.A + offsetof( T4Global, counters ), z, sizeof( z ) ) ;
-}
-
 // Create n seqsets in one go (one init launch).  handles[i] receives the new set.
 static int seqsets_create_impl( int n, int kmer_length, int hit_len_required, int consider_barcode, t4_seqset **handles ) ;
 
@@ -726,21 +665,9 @@ static int seqsets_create_impl( int n, int kmer_length, int hit_len_required, in
 	ip.footprint = (u32)fp ;
 	u64 base ;
 	r = arena_alloc( fp * n, &base ) ;
+	if ( !r ) r = launch_blocks( T4_KERNEL( t4_init_kernel, c_init_block ), n, 128, E.A, base, ip ) ;
+	if ( !r ) r = dsync() ;
 	if ( r ) return r ;
-#if T4_CUDA
-	t4_init_kernel<<<n, 128>>>( E.A, base, ip ) ;
-	CK( cudaGetLastError() ) ;
-	CK( cudaDeviceSynchronize() ) ;
-#else
-	T4Smem *sm = new T4Smem ;
-	for ( int b = 0 ; b < n ; ++b )
-	{
-		T4Ctx cx ;
-		cx.A = E.A ; cx.g = (T4Global *)E.A ; cx.st = 0 ; cx.sm = sm ; cx.cap = cx.g->cap ; cx.tid = 0 ; cx.nt = 1 ;
-		c_init_stream( cx, base + (u64)b * fp, ip ) ;
-	}
-	delete sm ;
-#endif
 	for ( int i = 0 ; i < n ; ++i )
 	{
 		t4_seqset *s = new t4_seqset ;
@@ -847,7 +774,7 @@ static int run_single( T4Op &op, const void *extra, size_t extraBytes, size_t ou
 		r = h2d( E.stage + sizeof( T4Op ), extra, extraBytes ) ;
 		if ( r ) return r ;
 	}
-	r = launch_ops( (T4Op *)E.stage, 1, 0 ) ;
+	r = launch_ops( T4K_STREAM, (T4Op *)E.stage, 1, 0 ) ;
 	if ( r ) return r ;
 	r = dsync() ;
 	if ( r ) return r ;
@@ -1174,39 +1101,20 @@ static int fetch_contigs( t4_seqset *s, HostContigs &hc )
 	hc.data.resize( tot ) ;
 	if ( tot == 0 )
 		return 0 ;
-#if T4_CUDA
-	size_t need = (size_t)n * sizeof( T4Contig ) + ( n + 1 ) * 8 + tot + 256 ;
-	r = ensure_stage( need ) ;
+	DevBuf m ;
+	T4Contig *dct ;
+	u64 *doff ;
+	char *dout ;
+	m.add( dct, (size_t)n * sizeof( T4Contig ) ) ;
+	m.add( doff, ( n + 1 ) * 8 ) ;
+	m.add( dout, tot ) ;
+	r = ensure_stage( m.bytes ) ;
 	if ( r ) return r ;
-	char *dct = E.stage ;
-	char *doff = dct + ( ( (size_t)n * sizeof( T4Contig ) + 63 ) & ~(size_t)63 ) ;
-	char *dout = doff + ( ( ( n + 1 ) * 8 + 63 ) & ~(size_t)63 ) ;
-	r = ensure_stage( ( dout - E.stage ) + tot ) ;
-	if ( r ) return r ;
-	dct = E.stage ;
-	doff = dct + ( ( (size_t)n * sizeof( T4Contig ) + 63 ) & ~(size_t)63 ) ;
-	dout = doff + ( ( ( n + 1 ) * 8 + 63 ) & ~(size_t)63 ) ;
-	r = h2d( dct, hc.ct.data(), (size_t)n * sizeof( T4Contig ) ) ;
-	if ( r ) return r ;
-	r = h2d( doff, hc.off.data(), ( n + 1 ) * 8 ) ;
-	if ( r ) return r ;
-	t4_gather_kernel<<<n, 128>>>( E.A, (const T4Contig *)dct, (const u64 *)doff, dout, n ) ;
-	CK( cudaGetLastError() ) ;
-	r = d2h( hc.data.data(), dout, tot ) ;
-	if ( r ) return r ;
-#else
-	for ( int i = 0 ; i < n ; ++i )
-	{
-		const T4Contig &k = hc.ct[i] ;
-		if ( !k.consOff )
-			continue ;
-		char *o = hc.data.data() + hc.off[i] ;
-		memcpy( o, E.A + k.consOff + k.lead, k.len ) ;
-		memcpy( o + k.len, E.A + k.pwOff + 16ull * k.lead, 16ull * k.len ) ;
-		memcpy( o + 17ull * k.len, E.A + k.nameOff, k.nameLen ) ;
-	}
-#endif
-	return 0 ;
+	m.place( E.stage ) ;
+	if ( ( r = h2d( dct, hc.ct.data(), (size_t)n * sizeof( T4Contig ) ) ) || ( r = h2d( doff, hc.off.data(), ( n + 1 ) * 8 ) )
+		|| ( r = launch_blocks( T4_KERNEL( t4_gather_kernel, t4_gather_block ), n, 128, E.A, dct, doff, dout, n ) ) )
+		return r ;
+	return d2h( hc.data.data(), dout, tot ) ;
 }
 
 // SeqSet::Output (SeqSet.hpp:10939-10994)
@@ -1411,37 +1319,22 @@ int T4_API( dp_pos_weight_batch )( int n, const int32_t *t_weights, const int64_
 	}
 	so[n] = tot ;
 	size_t szT = (size_t)t_off[n] * 16, szP = (size_t)p_off[n], szO = ( n + 1 ) * 8 ;
-	// one device allocation carved into the nine buffers: a single cleanup path whatever fails
-	auto al = []( size_t x ) { return ( x + 255 ) & ~(size_t)255 ; } ;
-	size_t oT = 0, oP = oT + al( szT + 16 ), oTo = oP + al( szP + 16 ), oPo = oTo + al( szO ), oA = oPo + al( szO ),
-		oAo = oA + al( (size_t)alignTot + 16 ), oS = oAo + al( szO ), oScr = oS + al( (size_t)n * 4 ), oSo = oScr + al( (size_t)tot + 16 ),
-		total = oSo + al( szO ) ;
-	void *base = 0 ;
-	r = dmalloc( &base, total ) ;
-	if ( r ) return r ;
-	struct Guard { void *p ; ~Guard() { dfree( p ) ; } } guard = { base } ;
-	char *B = (char *)base ;
-	void *dT = B + oT, *dP = B + oP, *dTo = B + oTo, *dPo = B + oPo, *dA = B + oA, *dAo = B + oAo, *dS = B + oS, *dScr = B + oScr, *dSo = B + oSo ;
-	if ( ( r = h2d( dT, t_weights, szT ) ) || ( r = h2d( dP, p, szP ) ) || ( r = h2d( dTo, t_off, szO ) ) || ( r = h2d( dPo, p_off, szO ) )
-		|| ( r = h2d( dAo, align_off, szO ) ) || ( r = h2d( dSo, so.data(), szO ) ) )
+	T4DpParams P ;
+	P.n = n ;
+	DevBuf m ;
+	int *dT ;
+	char *dP ;
+	i64 *dTo, *dPo, *dAo, *dSo ;
+	m.add( dT, szT + 16 ) ; m.add( dP, szP + 16 ) ; m.add( dTo, szO ) ; m.add( dPo, szO ) ; m.add( P.align, (size_t)alignTot + 16 ) ;
+	m.add( dAo, szO ) ; m.add( P.score, (size_t)n * 4 ) ; m.add( P.scratch, (size_t)tot + 16 ) ; m.add( dSo, szO ) ;
+	if ( ( r = m.alloc() ) )
 		return r ;
-#if T4_CUDA
-	t4_dp_kernel<<<( n + 63 ) / 64, 64>>>( n, (const int *)dT, (const i64 *)dTo, (const char *)dP, (const i64 *)dPo, (signed char *)dA,
-		(const i64 *)dAo, (int *)dS, (char *)dScr, (const i64 *)dSo ) ;
-	CK( cudaGetLastError() ) ;
-	CK( cudaDeviceSynchronize() ) ;
-#else
-	for ( int i = 0 ; i < n ; ++i )
-	{
-		int lent = (int)( t_off[i + 1] - t_off[i] ), lenp = (int)( p_off[i + 1] - p_off[i] ) ;
-		int d = lent > lenp ? lent - lenp : lenp - lent ;
-		int W = 2 * T4_DP_BAND + 3 + d ;
-		char *sc = (char *)dScr + so[i] ;
-		( (int *)dS )[i] = t4_dp_posweight( (const int *)dT + 4 * t_off[i], lent, (const char *)dP + p_off[i], lenp,
-			(signed char *)dA + align_off[i], (int *)sc, (unsigned char *)( sc + 8 * W ), 0 ) ;
-	}
-#endif
-	if ( ( r = d2h( align_out, dA, alignTot ) ) || ( r = d2h( score_out, dS, (size_t)n * 4 ) ) )
+	P.tw = dT ; P.p = dP ; P.tOff = dTo ; P.pOff = dPo ; P.alignOff = dAo ; P.scratchOff = dSo ;
+	if ( ( r = h2d( dT, t_weights, szT ) ) || ( r = h2d( dP, p, szP ) ) || ( r = h2d( dTo, t_off, szO ) ) || ( r = h2d( dPo, p_off, szO ) )
+		|| ( r = h2d( dAo, align_off, szO ) ) || ( r = h2d( dSo, so.data(), szO ) )
+		|| ( r = launch_items( T4_KERNEL( t4_dp_kernel, t4_dp_one ), P, n, 64 ) ) || ( r = dsync() ) )
+		return r ;
+	if ( ( r = d2h( align_out, P.align, alignTot ) ) || ( r = d2h( score_out, P.score, (size_t)n * 4 ) ) )
 		return r ;
 	return 0 ;
 }
@@ -1477,29 +1370,27 @@ int T4_API( dp_hot_path_batch )( int n, int variant, const int32_t *t_weights, c
 			alignTot = e ;
 	}
 	so[n] = tot ;
-	auto al = []( size_t x ) { return ( x + 255 ) & ~(size_t)255 ; } ;
 	size_t szT = (size_t)off[n] * 16, szP = (size_t)off[n], szO = (size_t)( n + 1 ) * 8 ;
-	size_t oT = 0, oP = oT + al( szT + 16 ), oOff = oP + al( szP + 16 ), oA = oOff + al( szO ), oAo = oA + al( (size_t)alignTot + 16 ),
-		oS = oAo + al( szO ), oScr = oS + al( (size_t)n * 4 ), oSo = oScr + al( (size_t)tot * 4 + 16 ), total = oSo + al( szO ) ;
-	void *base = 0 ;
-	r = dmalloc( &base, total ) ;
-	if ( r ) return r ;
-	struct Guard { void *p ; ~Guard() { dfree( p ) ; } } guard = { base } ;
-	char *B = (char *)base ;
-	if ( ( r = h2d( B + oT, t_weights, szT ) ) || ( r = h2d( B + oP, p, szP ) ) || ( r = h2d( B + oOff, off, szO ) )
-		|| ( r = h2d( B + oAo, align_off, szO ) ) || ( r = h2d( B + oSo, so.data(), szO ) ) )
+	DevBuf m ;
+	int *dT, *dS ;
+	char *dP ;
+	i64 *dOff, *dAo, *dSo ;
+	signed char *dA ;
+	u32 *dScr ;
+	m.add( dT, szT + 16 ) ; m.add( dP, szP + 16 ) ; m.add( dOff, szO ) ; m.add( dA, (size_t)alignTot + 16 ) ; m.add( dAo, szO ) ;
+	m.add( dS, (size_t)n * 4 ) ; m.add( dScr, (size_t)tot * 4 + 16 ) ; m.add( dSo, szO ) ;
+	if ( ( r = m.alloc() ) || ( r = h2d( dT, t_weights, szT ) ) || ( r = h2d( dP, p, szP ) ) || ( r = h2d( dOff, off, szO ) )
+		|| ( r = h2d( dAo, align_off, szO ) ) || ( r = h2d( dSo, so.data(), szO ) ) )
 		return r ;
 #if T4_CUDA
-	t4_dp_hot_kernel<<<n, 32>>>( n, variant, (const int *)( B + oT ), (const i64 *)( B + oOff ), B + oP, (signed char *)( B + oA ),
-		(const i64 *)( B + oAo ), (int *)( B + oS ), (u32 *)( B + oScr ), (const i64 *)( B + oSo ) ) ;
+	t4_dp_hot_kernel<<<n, 32>>>( n, variant, dT, dOff, dP, dA, dAo, dS, dScr, dSo ) ;
 	CK( cudaGetLastError() ) ;
 	CK( cudaDeviceSynchronize() ) ;
 #else
 	for ( int i = 0 ; i < n ; ++i )
-		( (int *)( B + oS ) )[i] = t4_dp_equal( (const int *)( B + oT ) + 4 * off[i], B + oP + off[i], (int)( off[i + 1] - off[i] ),
-			(signed char *)( B + oA ) + align_off[i], (u32 *)( B + oScr ) + so[i], false, 0 ) ;
+		dS[i] = t4_dp_equal( dT + 4 * off[i], dP + off[i], (int)( off[i + 1] - off[i] ), dA + align_off[i], dScr + so[i], false, 0 ) ;
 #endif
-	if ( ( r = d2h( align_out, B + oA, alignTot ) ) || ( r = d2h( score_out, B + oS, (size_t)n * 4 ) ) )
+	if ( ( r = d2h( align_out, dA, alignTot ) ) || ( r = d2h( score_out, dS, (size_t)n * 4 ) ) )
 		return r ;
 	return 0 ;
 }
@@ -1518,20 +1409,6 @@ static t4_workload *workload_upload_impl( const t4_read_desc *descs, int64_t n, 
 		npool += names[i] ;
 	}
 	noff[n_names] = (u32)npool.size() ;
-	auto al = []( size_t x ) { return ( x + 255 ) & ~(size_t)255 ; } ;
-	size_t oDesc = 0 ;
-	size_t oPool = oDesc + al( (size_t)n * sizeof( t4_read_desc ) ) ;
-	size_t oNames = oPool + al( pool_bytes + 16 ) ;
-	size_t oNoff = oNames + al( sizeof( T4Names ) ) ;
-	size_t oNpool = oNoff + al( ( n_names + 1 ) * 4 ) ;
-	size_t oRet = oNpool + al( npool.size() + 16 ) ;
-	size_t oStr = oRet + al( (size_t)n * 4 ) ;
-	size_t oResc = oStr + al( (size_t)n ) ;
-	size_t oRl = oResc + al( (size_t)n * 4 ) ;
-	size_t oGood = oRl + al( (size_t)n * 4 ) ;
-	size_t oInfo = oGood + al( (size_t)n ) ;
-	size_t oEv = oInfo + al( (size_t)n * 4 ) ;
-	size_t oOps = oEv + al( (size_t)n ) ;
 	// 2-bit packed copy of the reads, fixed stride (the longest supported read of the workload)
 	int maxLen = 0 ;
 	{
@@ -1554,103 +1431,71 @@ static t4_workload *workload_upload_impl( const t4_read_desc *descs, int64_t n, 
 				maxLen = part[t] ;
 	}
 	const u64 packStride = t4_pack_words( maxLen ) ;
-	size_t oPacked = oOps ;
-	size_t oOdd = oPacked + al( (size_t)n * packStride * 8 + 16 ) ;
-	size_t total = oOdd + 256 ;
-	void *p = 0 ;
+	t4_workload *w = new t4_workload ;
+	memset( w, 0, sizeof( *w ) ) ;
+	w->persistent = persistent ;
+	w->nDescs = n ;
+	w->poolBytes = pool_bytes ;
+	w->nNames = n_names ;
+	w->packStride = packStride ;
+	DevBuf m ;
+	u32 *dNoff, *dOdd ;
+	char *dNpool ;
+	m.add( w->descs, (size_t)n * sizeof( t4_read_desc ) ) ; m.add( w->pool, pool_bytes + 16 ) ; m.add( w->names, sizeof( T4Names ) ) ;
+	m.add( dNoff, ( n_names + 1 ) * 4 ) ; m.add( dNpool, npool.size() + 16 ) ; m.add( w->ret, (size_t)n * 4 ) ; m.add( w->strands, (size_t)n ) ;
+	m.add( w->rescue, (size_t)n * 4 ) ; m.add( w->rescueList, (size_t)n * 4 ) ; m.add( w->good, (size_t)n ) ; m.add( w->info, (size_t)n * 4 ) ;
+	m.add( w->events, (size_t)n ) ; m.add( w->packed, (size_t)n * packStride * 8 + 16 ) ; m.add( dOdd, 256 ) ;
 	if ( persistent )
 	{
-		if ( E.wlCap < total )
+		if ( E.wlCap < m.bytes )
 		{
 			if ( E.wl )
 				dfree( E.wl ) ;
 			E.wl = 0 ;
 			E.wlCap = 0 ;
-			size_t c = total + total / 4 ;
+			void *p = 0 ;
+			size_t c = m.bytes + m.bytes / 4 ;
 			if ( dmalloc( &p, c ) )
+			{
+				delete w ;
 				return 0 ;
+			}
 			E.wl = (char *)p ;
 			E.wlCap = c ;
 		}
-		p = E.wl ;
+		m.place( E.wl ) ;
 	}
-	else if ( dmalloc( &p, total ) )
-		return 0 ;
-	t4_workload *w = new t4_workload ;
-	memset( w, 0, sizeof( *w ) ) ;
-	w->persistent = persistent ;
-	w->buf = (char *)p ;
-	w->bytes = total ;
-	w->nDescs = n ;
-	w->poolBytes = pool_bytes ;
-	w->nNames = n_names ;
-	w->descs = (t4_read_desc *)( w->buf + oDesc ) ;
-	w->pool = w->buf + oPool ;
-	w->names = (T4Names *)( w->buf + oNames ) ;
-	w->ret = (int32_t *)( w->buf + oRet ) ;
-	w->strands = (int8_t *)( w->buf + oStr ) ;
-	w->rescue = (int32_t *)( w->buf + oResc ) ;
-	w->rescueList = (int32_t *)( w->buf + oRl ) ;
-	w->good = (int8_t *)( w->buf + oGood ) ;
-	w->info = (int32_t *)( w->buf + oInfo ) ;
-	w->events = (uint8_t *)( w->buf + oEv ) ;
-	w->packed = (u64 *)( w->buf + oPacked ) ;
-	w->packStride = packStride ;
-	w->usePacked = false ;
-	T4Names hn ;
-	hn.pool = (u64)(uintptr_t)( w->buf + oNpool ) ;
-	hn.off = (u64)(uintptr_t)( w->buf + oNoff ) ;
-	hn.n = n_names ;
-	hn.pad = 0 ;
-	if ( h2d( w->descs, descs, (size_t)n * sizeof( t4_read_desc ) ) || h2d( w->pool, read_pool, pool_bytes ) || h2d( w->names, &hn, sizeof( hn ) )
-		|| h2d( w->buf + oNoff, noff.data(), ( n_names + 1 ) * 4 ) || h2d( w->buf + oNpool, npool.data(), npool.size() ) )
+	else if ( m.alloc() )
 	{
-		if ( !persistent )
-			dfree( p ) ;
 		delete w ;
 		return 0 ;
 	}
+	T4Names hn ;
+	hn.pool = (u64)(uintptr_t)dNpool ;
+	hn.off = (u64)(uintptr_t)dNoff ;
+	hn.n = n_names ;
+	hn.pad = 0 ;
+	bool ok = !h2d( w->descs, descs, (size_t)n * sizeof( t4_read_desc ) ) && !h2d( w->pool, read_pool, pool_bytes ) && !h2d( w->names, &hn, sizeof( hn ) )
+		&& !h2d( dNoff, noff.data(), ( n_names + 1 ) * 4 ) && !h2d( dNpool, npool.data(), npool.size() ) ;
 	// pack on the device (the host API takes ASCII reads like the reference; they cross PCIe once, as ASCII)
 	u32 odd = 0 ;
-	u32 *dOdd = (u32 *)( w->buf + oOdd ) ;
-	bool ok = true ;
-	if ( n > 0 && packStride > 0 )
+	if ( ok && n > 0 && packStride > 0 )
 	{
-#if T4_CUDA
-		ok = cudaMemsetAsync( dOdd, 0, 4 ) == cudaSuccess ;
-		if ( ok )
-		{
-			const int wMax = (int)t4_pack_w( maxLen ) ;
-			const i64 threads = (i64)n * wMax ;
-			t4_pack_reads_kernel<<<(unsigned)( ( threads + 255 ) / 256 ), 256>>>( w->descs, n, w->pool, packStride, wMax, w->packed, dOdd ) ;
-			ok = cudaGetLastError() == cudaSuccess && cudaMemcpy( &odd, dOdd, 4, cudaMemcpyDeviceToHost ) == cudaSuccess ;
-		}
-#else
-		for ( int64_t r = 0 ; r < n ; ++r )
-		{
-			const int len = descs[r].len ;
-			if ( len <= 0 || len > T4_DEV_MAX_READ )
-				continue ;
-			const int W = (int)t4_pack_w( len ) ;
-			u64 *fw = w->packed + (u64)r * packStride, *rc = fw + W ;
-			u32 *nm = (u32 *)( fw + 2 * W ) ;
-			for ( int x = 0 ; x < W ; ++x )
-				t4_pack_word( w->pool + descs[r].seq_off, len, x, fw + x, rc + x, nm + x, &odd ) ;
-			if ( W & 1 )
-				nm[W] = 0 ;
-		}
-		(void)dOdd ;
-#endif
+		T4PackReadsParams P ;
+		P.descs = w->descs ; P.n = n ; P.pool = w->pool ; P.packStride = packStride ; P.wMax = (int)t4_pack_w( maxLen ) ;
+		P.packed = w->packed ; P.odd = dOdd ;
+		ok = !dzero( dOdd, 4 ) && !launch_items( T4_KERNEL( t4_pack_reads_kernel, t4_pack_read_word ), P, n * P.wMax, 256 ) && !d2h( &odd, dOdd, 4 ) ;
+		if ( !ok )
+			set_err( "packing the reads failed" ) ;
 	}
 	if ( !ok )
 	{
-		set_err( "packing the reads failed" ) ;
-		if ( !persistent )
-			dfree( p ) ;
 		delete w ;
 		return 0 ;
 	}
-	w->usePacked = ( odd == 0 && n > 0 && packStride > 0 && getenv( "T4_ASCII_READS" ) == NULL ) ;
+	w->buf = m.keep() ;
+	w->bytes = m.bytes ;
+	w->usePacked = ( odd == 0 && n > 0 && packStride > 0 ) ;
 	return w ;
 }
 
@@ -1739,12 +1584,9 @@ int T4_API( streams_run_resident )( t4_seqset *const *sets, int n_sets, const t4
 	r = ensure_ops( w, n_sets ) ;
 	if ( r ) return r ;
 	w->ran = true ;
-#if T4_CUDA
-	CK( cudaMemcpyAsync( w->ops, ops.data(), (size_t)n_sets * sizeof( T4Op ), cudaMemcpyHostToDevice, (cudaStream_t)cuda_stream ) ) ;
-#else
-	memcpy( w->ops, ops.data(), (size_t)n_sets * sizeof( T4Op ) ) ;
-#endif
-	return launch_ops( w->ops, n_sets, cuda_stream ) ;
+	r = h2d_async( w->ops, ops.data(), (size_t)n_sets * sizeof( T4Op ), cuda_stream ) ;
+	if ( r ) return r ;
+	return launch_ops( T4K_STREAM, w->ops, n_sets, cuda_stream ) ;
 }
 
 // ---- batch probe over frozen sets (t4_probe.cuh) ---------------------------------------------------
@@ -1766,29 +1608,19 @@ t4_hits *T4_API( hits_create )( int64_t max_reads, size_t max_hits )
 {
 	if ( ensure_up() || max_reads <= 0 )
 		return 0 ;
-	auto al = []( size_t x ) { return ( x + 255 ) & ~(size_t)255 ; } ;
-	size_t oKeys = 0, oOff = oKeys + al( max_hits * 8 + 16 ), oOrd = oOff + al( (size_t)max_reads * 8 ), oCnt = oOrd + al( (size_t)max_reads * 8 ),
-		oFl = oCnt + al( (size_t)max_reads * 4 ), oCtrl = oFl + al( (size_t)max_reads * 4 ), total = oCtrl + 256 ;
-	void *p = 0 ;
-	if ( dmalloc( &p, total ) )
-		return 0 ;
 	t4_hits *h = new t4_hits ;
 	memset( h, 0, sizeof( *h ) ) ;
 	h->maxReads = max_reads ;
 	h->keyCap = max_hits ;
-	h->buf = (char *)p ;
-	h->keys = (u64 *)( h->buf + oKeys ) ;
-	h->hitOff = (u64 *)( h->buf + oOff ) ;
-	h->ord = (u64 *)( h->buf + oOrd ) ;
-	h->hitCnt = (u32 *)( h->buf + oCnt ) ;
-	h->hitFlags = (u32 *)( h->buf + oFl ) ;
-	h->ctrl = (u64 *)( h->buf + oCtrl ) ;
-	if ( dzero( h->ctrl, 64 ) )
+	DevBuf m ;
+	m.add( h->keys, max_hits * 8 + 16 ) ; m.add( h->hitOff, (size_t)max_reads * 8 ) ; m.add( h->ord, (size_t)max_reads * 8 ) ;
+	m.add( h->hitCnt, (size_t)max_reads * 4 ) ; m.add( h->hitFlags, (size_t)max_reads * 4 ) ; m.add( h->ctrl, 256 ) ;
+	if ( m.alloc() || dzero( h->ctrl, 64 ) )
 	{
-		dfree( p ) ;
 		delete h ;
 		return 0 ;
 	}
+	h->buf = m.keep() ;
 	return h ;
 }
 
@@ -1860,21 +1692,16 @@ int T4_API( streams_get_hits )( t4_seqset *const *sets, int n_sets, t4_workload 
 	P.hitFlags = h->hitFlags ;
 	P.ctrl = h->ctrl ;
 	P.allowTotalSkip = allow_total_skip ? 1 : 0 ;
+	// registers bounded for 24 resident warps per SM, 2 directory probes in flight per lane
+	void ( *const probeKernel )( T4ProbeParams ) = t4_probe_kernel<24, 2> ;
 	static int probeBlocks = 0 ;
-	static void ( *probeKernel )( T4ProbeParams ) = 0 ;
 	const size_t probeSmem = sizeof( T4ProbeWarp ) * T4P_WARPS ;
 	if ( probeBlocks == 0 )
 	{
-		int perSm = 0, sms = 0 ;
-		const char *pv = getenv( "T4_PROBE_VARIANT" ) ;
-		// variants: resident warps per SM the registers are bounded for x directory probes in flight per lane (T4_PROBE_VARIANT=<warps><g>)
-		const int var = pv ? atoi( pv ) : 242 ;
-		probeKernel = var == 163 ? t4_probe_kernel<16, 3> : var == 203 ? t4_probe_kernel<20, 3> : var == 242 ? t4_probe_kernel<24, 2>
-			: var == 243 ? t4_probe_kernel<24, 3> : var == 162 ? t4_probe_kernel<16, 2> : var == 202 ? t4_probe_kernel<20, 2> : t4_probe_kernel<24, 2> ;
+		int perSm = 0 ;
 		CK( cudaFuncSetAttribute( probeKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)probeSmem ) ) ;
 		CK( cudaOccupancyMaxActiveBlocksPerMultiprocessor( &perSm, probeKernel, 32 * T4P_WARPS, probeSmem ) ) ;
-		CK( cudaDeviceGetAttribute( &sms, cudaDevAttrMultiProcessorCount, E.device ) ) ;
-		probeBlocks = ( perSm > 0 ? perSm : 1 ) * ( sms > 0 ? sms : 132 ) ; // persistent: one wave, a multiple of the SM count
+		probeBlocks = ( perSm > 0 ? perSm : 1 ) * E.sms ; // persistent: one wave, a multiple of the SM count
 	}
 	i64 need = ( n + T4P_WARPS - 1 ) / T4P_WARPS ;
 	int blocks = need < probeBlocks ? (int)need : probeBlocks ;
@@ -1890,8 +1717,7 @@ int T4_API( streams_get_hits )( t4_seqset *const *sets, int n_sets, t4_workload 
 	for ( int j = 0 ; j < n_sets ; ++j )
 		for ( i64 i = desc_off[j] ; i < desc_off[j + 1] ; ++i )
 		{
-			T4Ctx cx ;
-			cx.A = E.A ; cx.g = (T4Global *)E.A ; cx.st = (T4Stream *)( E.A + so[j] ) ; cx.sm = sm ; cx.cap = cx.g->cap ; cx.tid = 0 ; cx.nt = 1 ;
+			T4Ctx cx = t4_ctx( E.A, so[j], sm, 0, 1 ) ;
 			const t4_read_desc &d = w->descs[i] ;
 			h->hitOff[i] = top ;
 			h->hitCnt[i] = 0 ;
@@ -2046,15 +1872,7 @@ t4_assign *T4_API( streams_assign_reads )( t4_seqset *const *sets, int n_sets, t
 			return 0 ;
 		}
 	if ( n_workers <= 0 )
-	{
-#if T4_CUDA
-		int sms = 132 ;
-		cudaDeviceGetAttribute( &sms, cudaDevAttrMultiProcessorCount, E.device ) ;
-		n_workers = sms * T4_MIN_BLOCKS ; // one resident wave of the auxiliary kernel
-#else
-		n_workers = 2 ;
-#endif
-	}
+		n_workers = resident_workers() ;
 	t4_assign *a = new t4_assign ;
 	a->buf = 0 ; a->nDescs = n ; a->nSets = n_sets ; a->gen = g_gen ;
 	a->ext.assign( n_sets, (t4_seqset *)0 ) ;
@@ -2065,44 +1883,27 @@ t4_assign *T4_API( streams_assign_reads )( t4_seqset *const *sets, int n_sets, t
 		T4_API( assign_free )( a ) ;
 		return 0 ;
 	}
-	auto al = []( size_t x ) { return ( x + 255 ) & ~(size_t)255 ; } ;
 	const size_t nn = (size_t)( n > 0 ? n : 1 ) ;
-	size_t o = 0 ;
-	const size_t oP = o ; o += al( sizeof( T4AssignParams ) ) ;
-	const size_t oCur = o ; o += 256 ;
-	const size_t oOpsA = o ; o += al( (size_t)n_sets * sizeof( T4Op ) ) ;
-	const size_t oOpsB = o ; o += al( (size_t)n_workers * sizeof( T4Op ) ) ;
-	const size_t oOpsC = o ; o += al( (size_t)n_sets * sizeof( T4Op ) ) ;
-	const size_t oExt = o ; o += al( (size_t)n_sets * 8 ) ;
-	const size_t oSrc = o ; o += al( (size_t)n_sets * 8 ) ;
-	const size_t oDoff = o ; o += al( (size_t)( n_sets + 1 ) * 8 ) ;
-	const size_t oCnt = o ; o += al( (size_t)n_sets * 4 ) ;
-	const size_t oList = o ; o += al( nn * 4 ) ;
-	const size_t oLead = o ; o += al( nn * 4 ) ;
-	const size_t oSet = o ; o += al( nn * 4 ) ;
-	const size_t oAsg = o ; o += al( nn * 32 ) ;
-	const size_t oSim = o ; o += al( nn * 8 ) ;
-	void *p = 0 ;
-	if ( dmalloc( &p, o ) )
+	DevBuf m ;
+	T4Op *dOpsA, *dOpsB, *dOpsC ;
+	u64 *dExt, *dSrc ;
+	i64 *dDoff ;
+	int32_t *dCnt, *dList, *dLead, *dSet ;
+	m.add( a->dP, sizeof( T4AssignParams ) ) ; m.add( a->dCursor, 256 ) ; m.add( dOpsA, (size_t)n_sets * sizeof( T4Op ) ) ;
+	m.add( dOpsB, (size_t)n_workers * sizeof( T4Op ) ) ; m.add( dOpsC, (size_t)n_sets * sizeof( T4Op ) ) ; m.add( dExt, (size_t)n_sets * 8 ) ;
+	m.add( dSrc, (size_t)n_sets * 8 ) ; m.add( dDoff, (size_t)( n_sets + 1 ) * 8 ) ; m.add( dCnt, (size_t)n_sets * 4 ) ; m.add( dList, nn * 4 ) ;
+	m.add( dLead, nn * 4 ) ; m.add( dSet, nn * 4 ) ; m.add( a->dAssign, nn * 32 ) ; m.add( a->dSim, nn * 8 ) ;
+	if ( m.alloc() )
 	{
 		T4_API( assign_free )( a ) ;
 		return 0 ;
 	}
-	a->buf = (char *)p ;
-	a->dP = (T4AssignParams *)( a->buf + oP ) ;
-	a->dAssign = (int32_t *)( a->buf + oAsg ) ;
-	a->dSim = (double *)( a->buf + oSim ) ;
-	a->dCursor = (u64 *)( a->buf + oCur ) ;
 	T4AssignParams P ;
 	memset( &P, 0, sizeof( P ) ) ;
-	auto dp = [&]( size_t off ) { return (u64)(uintptr_t)( a->buf + off ) ; } ;
-	P.descs = (u64)(uintptr_t)w->descs ;
-	P.pool = (u64)(uintptr_t)w->pool ;
-	P.ret = (u64)(uintptr_t)w->ret ;
-	P.strands = (u64)(uintptr_t)w->strands ;
-	P.rescue = (u64)(uintptr_t)w->rescue ;
-	P.list = dp( oList ) ; P.leader = dp( oLead ) ; P.slotSet = dp( oSet ) ; P.assign = dp( oAsg ) ; P.sim = dp( oSim ) ;
-	P.extOff = dp( oExt ) ; P.srcOff = dp( oSrc ) ; P.descOff = dp( oDoff ) ; P.listCnt = dp( oCnt ) ; P.cursor = dp( oCur ) ;
+	auto dp = []( const void *q ) { return (u64)(uintptr_t)q ; } ;
+	P.descs = dp( w->descs ) ; P.pool = dp( w->pool ) ; P.ret = dp( w->ret ) ; P.strands = dp( w->strands ) ; P.rescue = dp( w->rescue ) ;
+	P.list = dp( dList ) ; P.leader = dp( dLead ) ; P.slotSet = dp( dSet ) ; P.assign = dp( a->dAssign ) ; P.sim = dp( a->dSim ) ;
+	P.extOff = dp( dExt ) ; P.srcOff = dp( dSrc ) ; P.descOff = dp( dDoff ) ; P.listCnt = dp( dCnt ) ; P.cursor = dp( a->dCursor ) ;
 	P.nDescs = n ; P.nSets = n_sets ; P.kmerLength = kmer_length ;
 	std::vector<u64> eo( n_sets ), so( n_sets ) ;
 	std::vector<T4Op> opsA( n_sets ), opsB( n_workers ), opsC( n_sets ) ;
@@ -2115,7 +1916,7 @@ t4_assign *T4_API( streams_assign_reads )( t4_seqset *const *sets, int n_sets, t
 		x.streamOff = eo[j] ;
 		x.op = T4_OP_ASSIGN_PREP ;
 		x.n = j ;
-		x.out = dp( oP ) ;
+		x.out = dp( a->dP ) ;
 		opsC[j] = x ;
 		opsC[j].op = T4_OP_ASSIGN_RECOMPUTE ;
 	}
@@ -2126,19 +1927,20 @@ t4_assign *T4_API( streams_assign_reads )( t4_seqset *const *sets, int n_sets, t
 		x.streamOff = a->workers[b]->off ;
 		x.op = T4_OP_ASSIGN ;
 		x.n = b ;
-		x.out = dp( oP ) ;
+		x.out = dp( a->dP ) ;
 	}
-	int r = h2d( a->buf + oP, &P, sizeof( P ) ) ;
-	if ( !r ) r = dzero( a->buf + oCur, 256 ) ;
-	if ( !r ) r = h2d( a->buf + oOpsA, opsA.data(), (size_t)n_sets * sizeof( T4Op ) ) ;
-	if ( !r ) r = h2d( a->buf + oOpsB, opsB.data(), (size_t)n_workers * sizeof( T4Op ) ) ;
-	if ( !r ) r = h2d( a->buf + oOpsC, opsC.data(), (size_t)n_sets * sizeof( T4Op ) ) ;
-	if ( !r ) r = h2d( a->buf + oExt, eo.data(), (size_t)n_sets * 8 ) ;
-	if ( !r ) r = h2d( a->buf + oSrc, so.data(), (size_t)n_sets * 8 ) ;
-	if ( !r ) r = h2d( a->buf + oDoff, desc_off, (size_t)( n_sets + 1 ) * 8 ) ;
-	if ( !r ) r = launch_aux_ops( (T4Op *)( a->buf + oOpsA ), n_sets, cuda_stream ) ;
-	if ( !r ) r = launch_aux_ops( (T4Op *)( a->buf + oOpsB ), n_workers, cuda_stream ) ;
-	if ( !r ) r = launch_aux_ops( (T4Op *)( a->buf + oOpsC ), n_sets, cuda_stream ) ;
+	int r = h2d( a->dP, &P, sizeof( P ) ) ;
+	if ( !r ) r = dzero( a->dCursor, 256 ) ;
+	if ( !r ) r = h2d( dOpsA, opsA.data(), (size_t)n_sets * sizeof( T4Op ) ) ;
+	if ( !r ) r = h2d( dOpsB, opsB.data(), (size_t)n_workers * sizeof( T4Op ) ) ;
+	if ( !r ) r = h2d( dOpsC, opsC.data(), (size_t)n_sets * sizeof( T4Op ) ) ;
+	if ( !r ) r = h2d( dExt, eo.data(), (size_t)n_sets * 8 ) ;
+	if ( !r ) r = h2d( dSrc, so.data(), (size_t)n_sets * 8 ) ;
+	if ( !r ) r = h2d( dDoff, desc_off, (size_t)( n_sets + 1 ) * 8 ) ;
+	if ( !r ) r = launch_ops( T4K_AUX, dOpsA, n_sets, cuda_stream ) ;
+	if ( !r ) r = launch_ops( T4K_AUX, dOpsB, n_workers, cuda_stream ) ;
+	if ( !r ) r = launch_ops( T4K_AUX, dOpsC, n_sets, cuda_stream ) ;
+	a->buf = m.keep() ;
 	if ( r )
 	{
 		T4_API( assign_free )( a ) ;
@@ -2370,36 +2172,37 @@ t4_refset *T4_API( refset_create_from_fa )( const char *fasta_path, int kmer_len
 		sp += seqs[i] ; np += names[i] ;
 		so[i + 1] = sp.size() ; no[i + 1] = np.size() ;
 	}
-	auto al = []( size_t x ) { return ( x + 255 ) & ~(size_t)255 ; } ;
-	const size_t oIn = 0, oOp = al( sizeof( T4RefInput ) ), oSp = oOp + al( sizeof( T4Op ) ), oSo = oSp + al( sp.size() + 16 ),
-		oNp = oSo + al( ( n + 1 ) * 8 ), oNo = oNp + al( np.size() + 16 ), total = oNo + al( ( n + 1 ) * 8 ) ;
-	void *p = 0 ;
-	if ( dmalloc( &p, total ) )
+	DevBuf m ;
+	T4RefInput *dIn ;
+	T4Op *dOp ;
+	char *dSp, *dNp ;
+	u64 *dSo, *dNo ;
+	m.add( dIn, sizeof( T4RefInput ) ) ; m.add( dOp, sizeof( T4Op ) ) ; m.add( dSp, sp.size() + 16 ) ; m.add( dSo, ( n + 1 ) * 8 ) ;
+	m.add( dNp, np.size() + 16 ) ; m.add( dNo, ( n + 1 ) * 8 ) ;
+	if ( m.alloc() )
 	{
 		T4_API( refset_free )( r ) ;
 		return 0 ;
 	}
-	char *b = (char *)p ;
 	T4RefInput in ;
 	memset( &in, 0, sizeof( in ) ) ;
-	in.seqPool = (u64)(uintptr_t)( b + oSp ) ; in.seqOff = (u64)(uintptr_t)( b + oSo ) ;
-	in.namePool = (u64)(uintptr_t)( b + oNp ) ; in.nameOff = (u64)(uintptr_t)( b + oNo ) ;
+	in.seqPool = (u64)(uintptr_t)dSp ; in.seqOff = (u64)(uintptr_t)dSo ;
+	in.namePool = (u64)(uintptr_t)dNp ; in.nameOff = (u64)(uintptr_t)dNo ;
 	in.n = n ;
 	T4Op op ;
 	memset( &op, 0, sizeof( op ) ) ;
 	op.streamOff = r->set->off ;
 	op.op = T4_OP_REF_INPUT ;
-	op.out = (u64)(uintptr_t)( b + oIn ) ;
-	int rc = h2d( b + oIn, &in, sizeof( in ) ) ;
-	if ( !rc ) rc = h2d( b + oOp, &op, sizeof( op ) ) ;
-	if ( !rc ) rc = h2d( b + oSp, sp.data(), sp.size() ) ;
-	if ( !rc ) rc = h2d( b + oSo, so.data(), ( n + 1 ) * 8 ) ;
-	if ( !rc ) rc = h2d( b + oNp, np.data(), np.size() ) ;
-	if ( !rc ) rc = h2d( b + oNo, no.data(), ( n + 1 ) * 8 ) ;
-	if ( !rc ) rc = launch_aux_ops( (T4Op *)( b + oOp ), 1, 0 ) ;
+	op.out = (u64)(uintptr_t)dIn ;
+	int rc = h2d( dIn, &in, sizeof( in ) ) ;
+	if ( !rc ) rc = h2d( dOp, &op, sizeof( op ) ) ;
+	if ( !rc ) rc = h2d( dSp, sp.data(), sp.size() ) ;
+	if ( !rc ) rc = h2d( dSo, so.data(), ( n + 1 ) * 8 ) ;
+	if ( !rc ) rc = h2d( dNp, np.data(), np.size() ) ;
+	if ( !rc ) rc = h2d( dNo, no.data(), ( n + 1 ) * 8 ) ;
+	if ( !rc ) rc = launch_ops( T4K_AUX, dOp, 1, 0 ) ;
 	if ( !rc ) rc = dsync() ;
-	if ( !rc ) rc = d2h( &op, b + oOp, sizeof( op ) ) ;
-	dfree( p ) ;
+	if ( !rc ) rc = d2h( &op, dOp, sizeof( op ) ) ;
 	if ( rc || op.ret != n )
 	{
 		if ( !rc )
@@ -2432,6 +2235,40 @@ int T4_API( refset_set_radius )( t4_refset *r, int radius )
 	return rc ? rc : put_field( r->set, offsetof( T4Stream, radius ), &radius, sizeof( int ) ) ;
 }
 
+// At least n scratch-only worker streams (the arena is a bump allocator: shells of an earlier count stay allocated
+// until t4_reset).
+static int refset_workers( t4_refset *r, int n )
+{
+	if ( (int)r->workers.size() >= n )
+		return 0 ;
+	for ( size_t i = 0 ; i < r->workers.size() ; ++i )
+		delete r->workers[i] ;
+	r->workers.assign( n, (t4_seqset *)0 ) ;
+	int rc = seqsets_create_impl( n, r->k, 31, 0, r->workers.data() ) ;
+	if ( rc )
+		r->workers.clear() ;
+	return rc ;
+}
+
+// Host read records: read i is pool[seq_off[i] .. + len[i]).  fn names the entry point in the message.
+static int check_records( const char *fn, size_t pool_bytes, const uint64_t *seq_off, const int32_t *len, i64 n )
+{
+	for ( i64 i = 0 ; i < n ; ++i )
+	{
+		if ( len[i] > T4_DEV_MAX_READ )
+		{
+			set_err( std::string( fn ) + ": read longer than the device limit" ) ;
+			return T4_E_UNSUPPORTED ;
+		}
+		if ( len[i] < 0 || seq_off[i] + (u64)len[i] > pool_bytes )
+		{
+			set_err( std::string( fn ) + ": record outside the pool" ) ;
+			return T4_E_INVAL ;
+		}
+	}
+	return 0 ;
+}
+
 // Device-pointer form of the scan: `pool`, `seq_off` (u64[n]), `len` (i32[n]), `strand_out` (i8[n]) and `low_out` (u8[n])
 // are DEVICE buffers, `ctrl` a device scratch of 64 bytes.  Asynchronous on cuda_stream.
 int T4_API( refset_scan_device )( t4_refset *r, const void *pool, const void *seq_off, const void *len, int64_t n, void *strand_out,
@@ -2445,28 +2282,9 @@ int T4_API( refset_scan_device )( t4_refset *r, const void *pool, const void *se
 		return T4_E_INVAL ;
 	}
 	if ( n_workers <= 0 )
-	{
-#if T4_CUDA
-		int sms = 132 ;
-		cudaDeviceGetAttribute( &sms, cudaDevAttrMultiProcessorCount, E.device ) ;
-		n_workers = sms * T4_MIN_BLOCKS ;
-#else
-		n_workers = 2 ;
-#endif
-	}
-	if ( (int)r->workers.size() != n_workers )
-	{
-		// (the arena is a bump allocator: shells of an earlier size stay allocated until t4_reset)
-		for ( size_t i = 0 ; i < r->workers.size() ; ++i )
-			delete r->workers[i] ;
-		r->workers.assign( n_workers, (t4_seqset *)0 ) ;
-		rc = seqsets_create_impl( n_workers, r->k, 31, 0, r->workers.data() ) ;
-		if ( rc )
-		{
-			r->workers.clear() ;
-			return rc ;
-		}
-	}
+		n_workers = resident_workers() ;
+	rc = refset_workers( r, n_workers ) ;
+	if ( rc ) return rc ;
 	T4ScanParams P ;
 	memset( &P, 0, sizeof( P ) ) ;
 	P.pool = (u64)(uintptr_t)pool ; P.seqOff = (u64)(uintptr_t)seq_off ; P.len = (u64)(uintptr_t)len ;
@@ -2496,18 +2314,10 @@ int T4_API( refset_scan_device )( t4_refset *r, const void *pool, const void *se
 		x.n = b ;
 		x.out = (u64)(uintptr_t)r->dbuf ;
 	}
-#if T4_CUDA
-	cudaStream_t cs = (cudaStream_t)cuda_stream ;
-	CK( cudaMemcpyAsync( r->dbuf, &P, sizeof( P ), cudaMemcpyHostToDevice, cs ) ) ;
-	CK( cudaMemcpyAsync( r->dbuf + 256, ops.data(), (size_t)n_workers * sizeof( T4Op ), cudaMemcpyHostToDevice, cs ) ) ;
-	CK( cudaMemsetAsync( ctrl, 0, 32, cs ) ) ;
-	CK( cudaStreamSynchronize( cs ) ) ; // P and ops are host temporaries
-#else
-	memcpy( r->dbuf, &P, sizeof( P ) ) ;
-	memcpy( r->dbuf + 256, ops.data(), (size_t)n_workers * sizeof( T4Op ) ) ;
-	memset( ctrl, 0, 32 ) ;
-#endif
-	return launch_aux_ops( (T4Op *)( r->dbuf + 256 ), n_workers, cuda_stream ) ;
+	if ( ( rc = h2d_async( r->dbuf, &P, sizeof( P ), cuda_stream ) ) || ( rc = h2d_async( r->dbuf + 256, ops.data(), (size_t)n_workers * sizeof( T4Op ), cuda_stream ) )
+		|| ( rc = dzero( ctrl, 32, cuda_stream ) ) )
+		return rc ;
+	return launch_ops( T4K_AUX, (T4Op *)( r->dbuf + 256 ), n_workers, cuda_stream ) ;
 }
 
 // Host form: for every read IsLowComplexity( read ) and refSet->HasHitInSet( read, 0 ) -- fastq-extractor keeps a read
@@ -2523,43 +2333,32 @@ int T4_API( refset_scan )( t4_refset *r, const char *read_pool, size_t pool_byte
 		set_err( "t4_refset_scan: bad argument" ) ;
 		return T4_E_INVAL ;
 	}
-	for ( i64 i = 0 ; i < n ; ++i )
-	{
-		if ( len[i] > T4_DEV_MAX_READ )
-		{
-			set_err( "t4_refset_scan: read longer than the device limit" ) ;
-			return T4_E_UNSUPPORTED ;
-		}
-		if ( len[i] < 0 || seq_off[i] + (u64)len[i] > pool_bytes )
-		{
-			set_err( "t4_refset_scan: record outside the pool" ) ;
-			return T4_E_INVAL ;
-		}
-	}
-	if ( n == 0 )
-		return 0 ;
-	auto al = []( size_t x ) { return ( x + 255 ) & ~(size_t)255 ; } ;
-	const size_t oPool = 0, oOff = al( pool_bytes + 16 ), oLen = oOff + al( (size_t)n * 8 ), oStr = oLen + al( (size_t)n * 4 ),
-		oLow = oStr + al( (size_t)n ), oCtrl = oLow + al( (size_t)n ), total = oCtrl + 256 ;
-	void *p = 0 ;
-	rc = dmalloc( &p, total ) ;
-	if ( rc ) return rc ;
-	char *b = (char *)p ;
-	rc = h2d( b + oPool, read_pool, pool_bytes ) ;
-	if ( !rc ) rc = h2d( b + oOff, seq_off, (size_t)n * 8 ) ;
-	if ( !rc ) rc = h2d( b + oLen, len, (size_t)n * 4 ) ;
-	if ( !rc ) rc = T4_API( refset_scan_device )( r, b + oPool, b + oOff, b + oLen, n, b + oStr, b + oLow, b + oCtrl, 0, 0 ) ;
+	rc = check_records( "t4_refset_scan", pool_bytes, seq_off, len, n ) ;
+	if ( rc || n == 0 )
+		return rc ;
+	DevBuf m ;
+	char *dPool ;
+	u64 *dOff, *dCtrl ;
+	int32_t *dLen ;
+	int8_t *dStr ;
+	uint8_t *dLow ;
+	m.add( dPool, pool_bytes + 16 ) ; m.add( dOff, (size_t)n * 8 ) ; m.add( dLen, (size_t)n * 4 ) ; m.add( dStr, (size_t)n ) ; m.add( dLow, (size_t)n ) ;
+	m.add( dCtrl, 256 ) ;
+	rc = m.alloc() ;
+	if ( !rc ) rc = h2d( dPool, read_pool, pool_bytes ) ;
+	if ( !rc ) rc = h2d( dOff, seq_off, (size_t)n * 8 ) ;
+	if ( !rc ) rc = h2d( dLen, len, (size_t)n * 4 ) ;
+	if ( !rc ) rc = T4_API( refset_scan_device )( r, dPool, dOff, dLen, n, dStr, dLow, dCtrl, 0, 0 ) ;
 	if ( !rc ) rc = dsync() ;
 	if ( !rc ) rc = T4_API( streams_error )( r->workers.data(), (int)r->workers.size() ) ;
-	if ( !rc && strand_out ) rc = d2h( strand_out, b + oStr, (size_t)n ) ;
-	if ( !rc && low_complexity_out ) rc = d2h( low_complexity_out, b + oLow, (size_t)n ) ;
+	if ( !rc && strand_out ) rc = d2h( strand_out, dStr, (size_t)n ) ;
+	if ( !rc && low_complexity_out ) rc = d2h( low_complexity_out, dLow, (size_t)n ) ;
 	if ( !rc && stats )
 	{
 		u64 c[4] ;
-		rc = d2h( c, b + oCtrl, sizeof( c ) ) ;
+		rc = d2h( c, dCtrl, sizeof( c ) ) ;
 		stats[0] = c[1] ; stats[1] = c[2] ;
 	}
-	dfree( p ) ;
 	return rc ;
 }
 
@@ -2581,54 +2380,41 @@ int T4_API( refset_get_overlaps )( t4_refset *r, const char *read, int32_t *over
 	if ( rc ) return rc ;
 	const int hMax = 1 << 16 ;
 	const size_t sb = t4_annot_scratch_bytes( hMax, st.nomatchGapLimit, T4_DEV_MAX_READ ) ;
-	auto al = []( size_t x ) { return ( x + 255 ) & ~(size_t)255 ; } ;
-	const size_t oOp = 0, oPar = al( sizeof( T4Op ) ), oRead = oPar + al( sizeof( T4RefOvlParams ) ), oOut = oRead + al( (size_t)len + 16 ),
-		oScr = oOut + al( (size_t)cap * 40 + 64 ), total = oScr + sb ;
-	void *p = 0 ;
-	rc = dmalloc( &p, total ) ;
+	DevBuf m ;
+	T4Op *dOp ;
+	T4RefOvlParams *dPar ;
+	char *dRead, *dOut, *dScr ;
+	m.add( dOp, sizeof( T4Op ) ) ; m.add( dPar, sizeof( T4RefOvlParams ) ) ; m.add( dRead, (size_t)len + 16 ) ; m.add( dOut, (size_t)cap * 40 + 64 ) ;
+	m.add( dScr, sb ) ;
+	rc = m.alloc() ;
 	if ( rc ) return rc ;
-	char *b = (char *)p ;
 	T4RefOvlParams P ;
 	memset( &P, 0, sizeof( P ) ) ;
-	P.scratch = (u64)(uintptr_t)( b + oScr ) ;
+	P.scratch = (u64)(uintptr_t)dScr ;
 	P.scratchBytes = sb ;
 	P.hMax = hMax ;
 	T4Op op ;
 	memset( &op, 0, sizeof( op ) ) ;
 	op.streamOff = r->set->off ;
 	op.op = T4_OP_REF_OVERLAPS ;
-	op.read = (u64)(uintptr_t)( b + oRead ) ;
+	op.read = (u64)(uintptr_t)dRead ;
 	op.len = len ;
-	op.out = (u64)(uintptr_t)( b + oOut ) ;
-	op.out2 = (u64)(uintptr_t)( b + oPar ) ;
+	op.out = (u64)(uintptr_t)dOut ;
+	op.out2 = (u64)(uintptr_t)dPar ;
 	op.outCap = cap ;
-	rc = h2d( b + oOp, &op, sizeof( op ) ) ;
-	if ( !rc ) rc = h2d( b + oPar, &P, sizeof( P ) ) ;
-	if ( !rc ) rc = h2d( b + oRead, read, (size_t)len + 1 ) ;
-	if ( !rc )
-	{
-#if T4_CUDA
-		t4_annot_kernel<<<1, E.nt>>>( E.A, (T4Op *)( b + oOp ) ) ;
-		if ( cudaGetLastError() != cudaSuccess )
-			rc = T4_E_CUDA ;
-#else
-		T4Smem *sm = new T4Smem ;
-		T4Ctx cx ;
-		cx.A = E.A ; cx.g = (T4Global *)E.A ; cx.st = (T4Stream *)( E.A + op.streamOff ) ; cx.sm = sm ; cx.cap = cx.g->cap ; cx.tid = 0 ; cx.nt = 1 ;
-		c_run_annot_op( cx, (T4Op *)( b + oOp ) ) ;
-		delete sm ;
-#endif
-	}
+	rc = h2d( dOp, &op, sizeof( op ) ) ;
+	if ( !rc ) rc = h2d( dPar, &P, sizeof( P ) ) ;
+	if ( !rc ) rc = h2d( dRead, read, (size_t)len + 1 ) ;
+	if ( !rc ) rc = launch_ops( T4K_ANNOT, dOp, 1, 0 ) ;
 	if ( !rc ) rc = dsync() ;
-	if ( !rc ) rc = d2h( &op, b + oOp, sizeof( op ) ) ;
+	if ( !rc ) rc = d2h( &op, dOp, sizeof( op ) ) ;
 	int n = op.ret ;
 	if ( !rc && n > 0 )
 	{
-		const int m = n < cap ? n : cap ;
-		rc = d2h( overlaps, b + oOut, (size_t)m * 32 ) ;
-		if ( !rc ) rc = d2h( similarity, b + oOut + (size_t)cap * 32, (size_t)m * 8 ) ;
+		const int k = n < cap ? n : cap ;
+		rc = d2h( overlaps, dOut, (size_t)k * 32 ) ;
+		if ( !rc ) rc = d2h( similarity, dOut + (size_t)cap * 32, (size_t)k * 8 ) ;
 	}
-	dfree( p ) ;
 	if ( rc ) return rc ;
 	if ( n < T4_E_BASE )
 		set_err( "t4_refset_get_overlaps: device error " + std::to_string( n ) ) ;
@@ -2649,61 +2435,37 @@ int T4_API( refset_annotate )( t4_refset *r, const char *read_pool, size_t pool_
 		set_err( "t4_refset_annotate: bad argument" ) ;
 		return T4_E_INVAL ;
 	}
-	for ( i64 i = 0 ; i < n ; ++i )
-	{
-		if ( len[i] > T4_DEV_MAX_READ )
-		{
-			set_err( "t4_refset_annotate: read longer than the device limit" ) ;
-			return T4_E_UNSUPPORTED ;
-		}
-		if ( len[i] < 0 || seq_off[i] + (u64)len[i] > pool_bytes )
-		{
-			set_err( "t4_refset_annotate: record outside the pool" ) ;
-			return T4_E_INVAL ;
-		}
-	}
-	if ( n == 0 )
-		return 0 ;
+	rc = check_records( "t4_refset_annotate", pool_bytes, seq_off, len, n ) ;
+	if ( rc || n == 0 )
+		return rc ;
 	T4Stream st ;
 	rc = get_stream( r->set, &st ) ;
 	if ( rc ) return rc ;
-#if T4_CUDA
-	int sms = 132 ;
-	cudaDeviceGetAttribute( &sms, cudaDevAttrMultiProcessorCount, E.device ) ;
-	int nw = sms * T4_MIN_BLOCKS ;
-#else
-	int nw = 2 ;
-#endif
+	int nw = resident_workers() ;
 	if ( (i64)nw > n )
 		nw = (int)n ;
-	if ( (int)r->workers.size() < nw )
-	{
-		for ( size_t i = 0 ; i < r->workers.size() ; ++i )
-			delete r->workers[i] ;
-		r->workers.assign( nw, (t4_seqset *)0 ) ;
-		rc = seqsets_create_impl( nw, r->k, 31, 0, r->workers.data() ) ;
-		if ( rc )
-		{
-			r->workers.clear() ;
-			return rc ;
-		}
-	}
-	const int hMax = 1 << 16 ; // hits of one read (contig) a worker has serial work space for: 16 MB per worker
-	auto al = []( size_t x ) { return ( x + 255 ) & ~(size_t)255 ; } ;
-	const size_t stride = al( t4_annot_scratch_bytes( hMax, st.nomatchGapLimit, T4_DEV_MAX_READ, st.nSeqs ) ) ;
-	const size_t oPar = 0, oOps = al( sizeof( T4AnnotParams ) ), oPool = oOps + al( (size_t)nw * sizeof( T4Op ) ), oOff = oPool + al( pool_bytes + 16 ),
-		oLen = oOff + al( (size_t)n * 8 ), oOut = oLen + al( (size_t)n * 4 ), oSim = oOut + al( (size_t)n * 4 * 8 * 4 ), oCtrl = oSim + al( (size_t)n * 4 * 8 ),
-		oScr = oCtrl + 256, total = oScr + stride * (size_t)nw ;
-	void *p = 0 ;
-	rc = dmalloc( &p, total ) ;
+	rc = refset_workers( r, nw ) ;
 	if ( rc ) return rc ;
-	char *b = (char *)p ;
+	const int hMax = 1 << 16 ; // hits of one read (contig) a worker has serial work space for: 16 MB per worker
+	const size_t stride = ( t4_annot_scratch_bytes( hMax, st.nomatchGapLimit, T4_DEV_MAX_READ, st.nSeqs ) + 255 ) & ~(size_t)255 ;
+	DevBuf m ;
+	T4AnnotParams *dPar ;
+	T4Op *dOps ;
+	char *dPool, *dScr ;
+	u64 *dOff, *dCtrl ;
+	int32_t *dLen, *dOut ;
+	double *dSim ;
+	m.add( dPar, sizeof( T4AnnotParams ) ) ; m.add( dOps, (size_t)nw * sizeof( T4Op ) ) ; m.add( dPool, pool_bytes + 16 ) ; m.add( dOff, (size_t)n * 8 ) ;
+	m.add( dLen, (size_t)n * 4 ) ; m.add( dOut, (size_t)n * 4 * 8 * 4 ) ; m.add( dSim, (size_t)n * 4 * 8 ) ; m.add( dCtrl, 256 ) ;
+	m.add( dScr, stride * (size_t)nw ) ;
+	rc = m.alloc() ;
+	if ( rc ) return rc ;
 	T4AnnotParams P ;
 	memset( &P, 0, sizeof( P ) ) ;
-	P.pool = (u64)(uintptr_t)( b + oPool ) ; P.seqOff = (u64)(uintptr_t)( b + oOff ) ; P.len = (u64)(uintptr_t)( b + oLen ) ;
-	P.out = (u64)(uintptr_t)( b + oOut ) ; P.sim = (u64)(uintptr_t)( b + oSim ) ; P.cursor = (u64)(uintptr_t)( b + oCtrl ) ;
+	P.pool = (u64)(uintptr_t)dPool ; P.seqOff = (u64)(uintptr_t)dOff ; P.len = (u64)(uintptr_t)dLen ;
+	P.out = (u64)(uintptr_t)dOut ; P.sim = (u64)(uintptr_t)dSim ; P.cursor = (u64)(uintptr_t)dCtrl ;
 	P.setOff = r->set->off ;
-	P.scratch = (u64)(uintptr_t)( b + oScr ) ; P.scratchStride = stride ;
+	P.scratch = (u64)(uintptr_t)dScr ; P.scratchStride = stride ;
 	P.n = n ; P.hMax = hMax ;
 	std::vector<T4Op> ops( nw ) ;
 	for ( int w = 0 ; w < nw ; ++w )
@@ -2712,37 +2474,19 @@ int T4_API( refset_annotate )( t4_refset *r, const char *read_pool, size_t pool_
 		ops[w].streamOff = r->workers[w]->off ;
 		ops[w].op = T4_OP_REF_ANNOTATE ;
 		ops[w].n = w ;
-		ops[w].out = (u64)(uintptr_t)( b + oPar ) ;
+		ops[w].out = (u64)(uintptr_t)dPar ;
 	}
-	rc = h2d( b + oPar, &P, sizeof( P ) ) ;
-	if ( !rc ) rc = h2d( b + oOps, ops.data(), (size_t)nw * sizeof( T4Op ) ) ;
-	if ( !rc ) rc = h2d( b + oPool, read_pool, pool_bytes ) ;
-	if ( !rc ) rc = h2d( b + oOff, seq_off, (size_t)n * 8 ) ;
-	if ( !rc ) rc = h2d( b + oLen, len, (size_t)n * 4 ) ;
-	if ( !rc ) rc = dzero( b + oCtrl, 64 ) ;
-	if ( !rc )
-	{
-#if T4_CUDA
-		t4_annot_kernel<<<nw, E.nt>>>( E.A, (T4Op *)( b + oOps ) ) ;
-		if ( cudaGetLastError() != cudaSuccess )
-			rc = T4_E_CUDA ;
-#else
-		T4Smem *sm = new T4Smem ;
-		for ( int w = 0 ; w < nw ; ++w )
-		{
-			T4Ctx cx ;
-			T4Op *o = (T4Op *)( b + oOps ) + w ;
-			cx.A = E.A ; cx.g = (T4Global *)E.A ; cx.st = (T4Stream *)( E.A + o->streamOff ) ; cx.sm = sm ; cx.cap = cx.g->cap ; cx.tid = 0 ; cx.nt = 1 ;
-			c_run_annot_op( cx, o ) ;
-		}
-		delete sm ;
-#endif
-	}
+	rc = h2d( dPar, &P, sizeof( P ) ) ;
+	if ( !rc ) rc = h2d( dOps, ops.data(), (size_t)nw * sizeof( T4Op ) ) ;
+	if ( !rc ) rc = h2d( dPool, read_pool, pool_bytes ) ;
+	if ( !rc ) rc = h2d( dOff, seq_off, (size_t)n * 8 ) ;
+	if ( !rc ) rc = h2d( dLen, len, (size_t)n * 4 ) ;
+	if ( !rc ) rc = dzero( dCtrl, 64 ) ;
+	if ( !rc ) rc = launch_ops( T4K_ANNOT, dOps, nw, 0 ) ;
 	if ( !rc ) rc = dsync() ;
 	if ( !rc ) rc = T4_API( streams_error )( r->workers.data(), nw ) ;
-	if ( !rc ) rc = d2h( gene_overlaps, b + oOut, (size_t)n * 4 * 8 * 4 ) ;
-	if ( !rc ) rc = d2h( similarity, b + oSim, (size_t)n * 4 * 8 ) ;
-	dfree( p ) ;
+	if ( !rc ) rc = d2h( gene_overlaps, dOut, (size_t)n * 4 * 8 * 4 ) ;
+	if ( !rc ) rc = d2h( similarity, dSim, (size_t)n * 4 * 8 ) ;
 	return rc ;
 }
 
@@ -2776,42 +2520,29 @@ int T4_API( sort_reads )( const char *read_pool, size_t pool_bytes, const uint64
 		r.readOff = seq_off[i] ; r.idOff = id_off[i] ; r.idLen = (int32_t)( id_off[i + 1] - id_off[i] ) ; r.pad = 0 ;
 		idx[(size_t)i] = i ;
 	}
-	auto al = []( size_t x ) { return ( x + 255 ) & ~(size_t)255 ; } ;
-	const size_t oRec = 0, oPool = al( (size_t)n * sizeof( T4SortRec ) ), oId = oPool + al( pool_bytes + 16 ), oA = oId + al( id_pool_bytes + 16 ),
-		oB = oA + al( (size_t)n * 8 ), total = oB + al( (size_t)n * 8 ) ;
-	void *p = 0 ;
-	rc = dmalloc( &p, total ) ;
-	if ( rc ) return rc ;
-	char *b = (char *)p ;
-	rc = h2d( b + oRec, recs.data(), (size_t)n * sizeof( T4SortRec ) ) ;
-	if ( !rc ) rc = h2d( b + oPool, read_pool, pool_bytes ) ;
-	if ( !rc ) rc = h2d( b + oId, id_pool, id_pool_bytes ) ;
-	if ( !rc ) rc = h2d( b + oA, idx.data(), (size_t)n * 8 ) ;
+	DevBuf m ;
+	T4SortRec *dRec ;
+	char *dPool, *dId ;
+	i64 *from, *to ;
+	m.add( dRec, (size_t)n * sizeof( T4SortRec ) ) ; m.add( dPool, pool_bytes + 16 ) ; m.add( dId, id_pool_bytes + 16 ) ; m.add( from, (size_t)n * 8 ) ;
+	m.add( to, (size_t)n * 8 ) ;
+	rc = m.alloc() ;
+	if ( !rc ) rc = h2d( dRec, recs.data(), (size_t)n * sizeof( T4SortRec ) ) ;
+	if ( !rc ) rc = h2d( dPool, read_pool, pool_bytes ) ;
+	if ( !rc ) rc = h2d( dId, id_pool, id_pool_bytes ) ;
+	if ( !rc ) rc = h2d( from, idx.data(), (size_t)n * 8 ) ;
 	T4SortParams P ;
 	memset( &P, 0, sizeof( P ) ) ;
-	P.recs = (u64)(uintptr_t)( b + oRec ) ; P.pool = (u64)(uintptr_t)( b + oPool ) ; P.idPool = (u64)(uintptr_t)( b + oId ) ;
+	P.recs = (u64)(uintptr_t)dRec ; P.pool = (u64)(uintptr_t)dPool ; P.idPool = (u64)(uintptr_t)dId ;
 	P.n = n ;
-	size_t from = oA, to = oB ;
 	for ( i64 w = 1 ; !rc && w < n ; w *= 2 )
 	{
-		P.src = (u64)(uintptr_t)( b + from ) ; P.dst = (u64)(uintptr_t)( b + to ) ; P.width = w ;
-#if T4_CUDA
-		const int threads = 256 ;
-		i64 blocks = ( n + threads - 1 ) / threads ;
-		if ( blocks > 132 * 16 )
-			blocks = 132 * 16 ;
-		t4_readsort_kernel<<<(int)blocks, threads>>>( P ) ;
-		if ( cudaGetLastError() != cudaSuccess )
-			rc = T4_E_CUDA ;
-#else
-		for ( i64 i = 0 ; i < n ; ++i )
-			t4_sort_merge_one( P, i ) ;
-#endif
-		const size_t t = from ; from = to ; to = t ;
+		P.src = (u64)(uintptr_t)from ; P.dst = (u64)(uintptr_t)to ; P.width = w ;
+		rc = launch_items( T4_KERNEL( t4_readsort_kernel, t4_sort_merge_one ), P, n, 256 ) ;
+		i64 *t = from ; from = to ; to = t ;
 	}
 	if ( !rc ) rc = dsync() ;
-	if ( !rc ) rc = d2h( order, b + from, (size_t)n * 8 ) ;
-	dfree( p ) ;
+	if ( !rc ) rc = d2h( order, from, (size_t)n * 8 ) ;
 	return rc ;
 }
 
@@ -2837,46 +2568,32 @@ int T4_API( mate_overlap_batch )( const char *read_pool, size_t pool_bytes, cons
 		}
 	if ( n == 0 )
 		return 0 ;
-	auto al = []( size_t x ) { return ( x + 255 ) & ~(size_t)255 ; } ;
-	const size_t n8 = al( (size_t)n * 8 ), n4 = al( (size_t)n * 4 ), n1 = al( (size_t)n ) ;
-	const size_t oPool = 0, oFo = al( pool_bytes + 16 ), oSo = oFo + n8, oFl = oSo + n8, oSl = oFl + n4, oMo = oSl + n4, oCt = oMo + n4,
-		oOs = oCt + n1, oOf = oOs + n4, oBm = oOf + n4, total = oBm + n4 ;
-	void *p = 0 ;
-	rc = dmalloc( &p, total ) ;
-	if ( rc ) return rc ;
-	char *b = (char *)p ;
-	rc = h2d( b + oPool, read_pool, pool_bytes ) ;
-	if ( !rc ) rc = h2d( b + oFo, f_off, (size_t)n * 8 ) ;
-	if ( !rc ) rc = h2d( b + oSo, s_off, (size_t)n * 8 ) ;
-	if ( !rc ) rc = h2d( b + oFl, f_len, (size_t)n * 4 ) ;
-	if ( !rc ) rc = h2d( b + oSl, s_len, (size_t)n * 4 ) ;
-	if ( !rc ) rc = h2d( b + oMo, min_overlap, (size_t)n * 4 ) ;
-	if ( !rc ) rc = h2d( b + oCt, check_tandem, (size_t)n ) ;
+	DevBuf m ;
+	char *dPool ;
+	u64 *dFo, *dSo ;
+	int32_t *dFl, *dSl, *dMo, *dOs, *dOf, *dBm ;
+	uint8_t *dCt ;
+	m.add( dPool, pool_bytes + 16 ) ; m.add( dFo, (size_t)n * 8 ) ; m.add( dSo, (size_t)n * 8 ) ; m.add( dFl, (size_t)n * 4 ) ; m.add( dSl, (size_t)n * 4 ) ;
+	m.add( dMo, (size_t)n * 4 ) ; m.add( dCt, (size_t)n ) ; m.add( dOs, (size_t)n * 4 ) ; m.add( dOf, (size_t)n * 4 ) ; m.add( dBm, (size_t)n * 4 ) ;
+	rc = m.alloc() ;
+	if ( !rc ) rc = h2d( dPool, read_pool, pool_bytes ) ;
+	if ( !rc ) rc = h2d( dFo, f_off, (size_t)n * 8 ) ;
+	if ( !rc ) rc = h2d( dSo, s_off, (size_t)n * 8 ) ;
+	if ( !rc ) rc = h2d( dFl, f_len, (size_t)n * 4 ) ;
+	if ( !rc ) rc = h2d( dSl, s_len, (size_t)n * 4 ) ;
+	if ( !rc ) rc = h2d( dMo, min_overlap, (size_t)n * 4 ) ;
+	if ( !rc ) rc = h2d( dCt, check_tandem, (size_t)n ) ;
 	T4MateParams P ;
 	memset( &P, 0, sizeof( P ) ) ;
-	auto dp = [&]( size_t off ) { return (u64)(uintptr_t)( b + off ) ; } ;
-	P.pool = dp( oPool ) ; P.fOff = dp( oFo ) ; P.sOff = dp( oSo ) ; P.fLen = dp( oFl ) ; P.sLen = dp( oSl ) ; P.minOverlap = dp( oMo ) ;
-	P.checkTandem = dp( oCt ) ; P.overlapSize = dp( oOs ) ; P.offset = dp( oOf ) ; P.bestMatchCnt = dp( oBm ) ;
+	auto dp = []( const void *q ) { return (u64)(uintptr_t)q ; } ;
+	P.pool = dp( dPool ) ; P.fOff = dp( dFo ) ; P.sOff = dp( dSo ) ; P.fLen = dp( dFl ) ; P.sLen = dp( dSl ) ; P.minOverlap = dp( dMo ) ;
+	P.checkTandem = dp( dCt ) ; P.overlapSize = dp( dOs ) ; P.offset = dp( dOf ) ; P.bestMatchCnt = dp( dBm ) ;
 	P.n = n ;
-	if ( !rc )
-	{
-#if T4_CUDA
-		i64 blocks = ( n + 127 ) / 128 ;
-		if ( blocks > 132 * 16 )
-			blocks = 132 * 16 ;
-		t4_mate_overlap_kernel<<<(int)blocks, 128>>>( P ) ;
-		if ( cudaGetLastError() != cudaSuccess )
-			rc = T4_E_CUDA ;
-#else
-		for ( i64 i = 0 ; i < n ; ++i )
-			t4_mate_overlap_one( P, i ) ;
-#endif
-	}
+	if ( !rc ) rc = launch_items( T4_KERNEL( t4_mate_overlap_kernel, t4_mate_overlap_one ), P, n, 128 ) ;
 	if ( !rc ) rc = dsync() ;
-	if ( !rc ) rc = d2h( overlap_size, b + oOs, (size_t)n * 4 ) ;
-	if ( !rc ) rc = d2h( offset, b + oOf, (size_t)n * 4 ) ;
-	if ( !rc ) rc = d2h( best_match_cnt, b + oBm, (size_t)n * 4 ) ;
-	dfree( p ) ;
+	if ( !rc ) rc = d2h( overlap_size, dOs, (size_t)n * 4 ) ;
+	if ( !rc ) rc = d2h( offset, dOf, (size_t)n * 4 ) ;
+	if ( !rc ) rc = d2h( best_match_cnt, dBm, (size_t)n * 4 ) ;
 	return rc ;
 }
 
@@ -2894,10 +2611,8 @@ int T4_API( test_lis )( const int32_t *a, const int32_t *b, int n, int32_t *out_
 static int kc_launch( const T4KcParams &P, int stats, void *stream )
 {
 #if T4_CUDA
-	int sms = 132 ;
-	cudaDeviceGetAttribute( &sms, cudaDevAttrMultiProcessorCount, E.device ) ;
 	CK( cudaMemsetAsync( (void *)(uintptr_t)P.ctrl, 0, 8, (cudaStream_t)stream ) ) ; // the read cursor
-	t4_kcount_kernel<<<sms * 10, T4_MAX_NT, 0, (cudaStream_t)stream>>>( P, stats ) ; // 40 warps per SM (21 KB of shared memory per CTA)
+	t4_kcount_kernel<<<E.sms * 10, T4_MAX_NT, 0, (cudaStream_t)stream>>>( P, stats ) ; // 40 warps per SM (21 KB of shared memory per CTA)
 	CK( cudaGetLastError() ) ;
 #else
 	*(u64 *)(uintptr_t)P.ctrl = 0 ;
@@ -2953,12 +2668,8 @@ int T4_API( kmer_count_stats_device )( const void *pool, const void *qual, const
 	P.newLen = (u64)(uintptr_t)new_len ;
 	P.n = n ;
 	P.k = kmer_length ;
-#if T4_CUDA
-	CK( cudaMemsetAsync( table, 0, cap * 12 + 64, (cudaStream_t)cuda_stream ) ) ;
-#else
-	memset( table, 0, cap * 12 + 64 ) ;
-#endif
-	r = kc_launch( P, 0, cuda_stream ) ;
+	r = dzero( table, cap * 12 + 64, cuda_stream ) ;
+	if ( !r ) r = kc_launch( P, 0, cuda_stream ) ;
 	if ( !r ) r = kc_launch( P, 1, cuda_stream ) ;
 	return r ;
 }
@@ -2991,51 +2702,38 @@ int T4_API( kmer_count_stats )( const char *read_pool, const char *qual_pool, si
 		set_err( "t4_kmer_count_stats: bad argument" ) ;
 		return T4_E_INVAL ;
 	}
+	r = check_records( "t4_kmer_count_stats", pool_bytes, seq_off, len, n ) ;
+	if ( r || n == 0 )
+		return r ;
 	u64 inst = 0 ;
 	for ( i64 i = 0 ; i < n ; ++i )
-	{
-		if ( len[i] > T4_DEV_MAX_READ )
-		{
-			set_err( "t4_kmer_count_stats: read longer than the device limit" ) ;
-			return T4_E_UNSUPPORTED ;
-		}
-		if ( len[i] < 0 || seq_off[i] + (u64)len[i] > pool_bytes )
-		{
-			set_err( "t4_kmer_count_stats: record outside the pool" ) ;
-			return T4_E_INVAL ;
-		}
 		if ( len[i] >= kmer_length )
 			inst += (u64)( len[i] - kmer_length + 1 ) ;
-	}
-	if ( n == 0 )
-		return 0 ;
 	const size_t tb = T4_API( kmer_count_table_bytes )( (int64_t)inst ) ;
-	auto al = []( size_t x ) { return ( x + 255 ) & ~(size_t)255 ; } ;
-	const size_t oPool = 0, oQual = al( pool_bytes + 16 ), oOff = oQual + ( qual_pool ? al( pool_bytes + 16 ) : 0 ), oLen = oOff + al( (size_t)n * 8 ),
-		oMin = oLen + al( (size_t)n * 4 ), oMed = oMin + al( (size_t)n * 4 ), oAvg = oMed + al( (size_t)n * 4 ), oNew = oAvg + al( (size_t)n * 4 ),
-		oTab = oNew + al( (size_t)n * 4 ), total = oTab + tb ;
-	void *p = 0 ;
-	r = dmalloc( &p, total ) ;
-	if ( r ) return r ;
-	char *b = (char *)p ;
-	r = h2d( b + oPool, read_pool, pool_bytes ) ;
-	if ( !r && qual_pool ) r = h2d( b + oQual, qual_pool, pool_bytes ) ;
-	if ( !r ) r = h2d( b + oOff, seq_off, (size_t)n * 8 ) ;
-	if ( !r ) r = h2d( b + oLen, len, (size_t)n * 4 ) ;
-	if ( !r ) r = T4_API( kmer_count_stats_device )( b + oPool, qual_pool ? b + oQual : 0, b + oOff, b + oLen, n, kmer_length, b + oTab, tb, b + oMin,
-		b + oMed, b + oAvg, b + oNew, 0 ) ;
+	DevBuf m ;
+	char *dPool, *dQual, *dTab ;
+	u64 *dOff ;
+	int32_t *dLen, *dMin, *dMed, *dNew ;
+	float *dAvg ;
+	m.add( dPool, pool_bytes + 16 ) ; m.add( dQual, qual_pool ? pool_bytes + 16 : 0 ) ; m.add( dOff, (size_t)n * 8 ) ; m.add( dLen, (size_t)n * 4 ) ;
+	m.add( dMin, (size_t)n * 4 ) ; m.add( dMed, (size_t)n * 4 ) ; m.add( dAvg, (size_t)n * 4 ) ; m.add( dNew, (size_t)n * 4 ) ; m.add( dTab, tb ) ;
+	r = m.alloc() ;
+	if ( !r ) r = h2d( dPool, read_pool, pool_bytes ) ;
+	if ( !r && qual_pool ) r = h2d( dQual, qual_pool, pool_bytes ) ;
+	if ( !r ) r = h2d( dOff, seq_off, (size_t)n * 8 ) ;
+	if ( !r ) r = h2d( dLen, len, (size_t)n * 4 ) ;
+	if ( !r ) r = T4_API( kmer_count_stats_device )( dPool, qual_pool ? dQual : 0, dOff, dLen, n, kmer_length, dTab, tb, dMin, dMed, dAvg, dNew, 0 ) ;
 	u64 st[4] = { 0, 0, 0, 0 } ;
-	if ( !r ) r = T4_API( kmer_count_table_stats )( b + oTab, tb, st ) ;
+	if ( !r ) r = T4_API( kmer_count_table_stats )( dTab, tb, st ) ;
 	if ( !r && st[3] )
 	{
 		set_err( "t4_kmer_count_stats: count table overflow" ) ;
 		r = T4_E_INTERNAL ;
 	}
-	if ( !r && min_cnt ) r = d2h( min_cnt, b + oMin, (size_t)n * 4 ) ;
-	if ( !r && median_cnt ) r = d2h( median_cnt, b + oMed, (size_t)n * 4 ) ;
-	if ( !r && avg_cnt ) r = d2h( avg_cnt, b + oAvg, (size_t)n * 4 ) ;
-	if ( !r && new_len ) r = d2h( new_len, b + oNew, (size_t)n * 4 ) ;
-	dfree( p ) ;
+	if ( !r && min_cnt ) r = d2h( min_cnt, dMin, (size_t)n * 4 ) ;
+	if ( !r && median_cnt ) r = d2h( median_cnt, dMed, (size_t)n * 4 ) ;
+	if ( !r && avg_cnt ) r = d2h( avg_cnt, dAvg, (size_t)n * 4 ) ;
+	if ( !r && new_len ) r = d2h( new_len, dNew, (size_t)n * 4 ) ;
 	return r ;
 }
 
@@ -3087,37 +2785,13 @@ int T4_API( streams_pack_contigs )( t4_seqset *const *sets, int n_sets, void *de
 	}
 	int r = dsync() ;
 	if ( r ) return r ;
-#if T4_CUDA
 	r = ensure_stage( (size_t)n_sets * 32 + 256 ) ;
 	if ( r ) return r ;
 	u64 *dSo = (u64 *)E.stage, *dSz = dSo + n_sets, *dCnt = dSz + n_sets, *dOff = dCnt + n_sets ;
-	r = h2d( dSo, so.data(), (size_t)n_sets * 8 ) ;
-	if ( r ) return r ;
-	t4_pack_size_kernel<<<n_sets, 128>>>( E.A, dSo, dSz, dCnt ) ;
-	CK( cudaGetLastError() ) ;
-	r = d2h( sizes.data(), dSz, (size_t)n_sets * 8 ) ;
-	if ( r ) return r ;
-	r = d2h( counts.data(), dCnt, (size_t)n_sets * 8 ) ;
-	if ( r ) return r ;
-#else
-	for ( int j = 0 ; j < n_sets ; ++j )
-	{
-		const T4Stream *st = (const T4Stream *)( E.A + so[j] ) ;
-		T4Contig *ct = (T4Contig *)( E.A + st->seqsOff ) ;
-		sizes[j] = counts[j] = 0 ;
-		for ( int i = 0 ; i < st->nSeqs ; ++i )
-			if ( ct[i].consOff )
-			{
-				const int *pw = (const int *)( E.A + ct[i].pwOff + 16ull * ct[i].lead ) ;
-				int wide = 0 ;
-				for ( int x = 0 ; x < 4 * ct[i].len ; ++x )
-					wide |= ( (unsigned)pw[x] > 65535u ) ;
-				ct[i].packNarrow = wide ? 0 : 1 ;
-				sizes[j] += t4_pack_record_bytes( ct[i] ) ;
-				++counts[j] ;
-			}
-	}
-#endif
+	if ( ( r = h2d( dSo, so.data(), (size_t)n_sets * 8 ) )
+		|| ( r = launch_blocks( T4_KERNEL( t4_pack_size_kernel, t4_pack_size_block ), n_sets, 128, E.A, dSo, dSz, dCnt ) )
+		|| ( r = d2h( sizes.data(), dSz, (size_t)n_sets * 8 ) ) || ( r = d2h( counts.data(), dCnt, (size_t)n_sets * 8 ) ) )
+		return r ;
 	u64 tot = 0, n = 0 ;
 	for ( int j = 0 ; j < n_sets ; ++j )
 	{
@@ -3134,50 +2808,9 @@ int T4_API( streams_pack_contigs )( t4_seqset *const *sets, int n_sets, void *de
 		set_err( "pack buffer too small" ) ;
 		return T4_E_INVAL ;
 	}
-#if T4_CUDA
 	r = h2d( dOff, off.data(), (size_t)n_sets * 8 ) ;
 	if ( r ) return r ;
-	t4_pack_kernel<<<n_sets, 128>>>( E.A, dSo, dOff, (char *)dev_buf ) ;
-	CK( cudaGetLastError() ) ;
-#else
-	for ( int j = 0 ; j < n_sets ; ++j )
-	{
-		const T4Stream *st = (const T4Stream *)( E.A + so[j] ) ;
-		const T4Contig *ct = (const T4Contig *)( E.A + st->seqsOff ) ;
-		u64 o = off[j] ;
-		for ( int i = 0 ; i < st->nSeqs ; ++i )
-		{
-			const T4Contig &k = ct[i] ;
-			if ( !k.consOff )
-				continue ;
-			u64 rb = t4_pack_record_bytes( k ) ;
-			char *rec = (char *)dev_buf + o ;
-			memset( rec, 0, rb ) ;
-			u32 *h = (u32 *)rec ;
-			h[0] = j ; h[1] = (u32)i ; h[2] = (u32)k.len ; h[3] = (u32)k.nameLen ; h[4] = (u32)k.barcode ; h[5] = (u32)k.numRead ; h[6] = (u32)rb ;
-			h[7] = k.packNarrow ? 1u : 0u ;
-			memcpy( rec + 32, E.A + k.consOff + k.lead, k.len ) ;
-			if ( k.packNarrow )
-			{
-				const int *pw = (const int *)( E.A + k.pwOff + 16ull * k.lead ) ;
-				unsigned char *d = (unsigned char *)rec + 32 + k.len ;
-				for ( int x = 0 ; x < 4 * k.len ; ++x )
-				{
-					d[2 * x] = (unsigned char)( (unsigned)pw[x] & 255u ) ;
-					d[2 * x + 1] = (unsigned char)( (unsigned)pw[x] >> 8 ) ;
-				}
-				memcpy( rec + 32 + 9ull * k.len, E.A + k.nameOff, k.nameLen ) ;
-			}
-			else
-			{
-				memcpy( rec + 32 + k.len, E.A + k.pwOff + 16ull * k.lead, 16ull * k.len ) ;
-				memcpy( rec + 32 + 17ull * k.len, E.A + k.nameOff, k.nameLen ) ;
-			}
-			o += rb ;
-		}
-	}
-#endif
-	return 0 ;
+	return launch_blocks( T4_KERNEL( t4_pack_kernel, t4_pack_block ), n_sets, 128, E.A, dSo, dOff, (char *)dev_buf ) ;
 }
 
 // Diagnostics: SM clock cycles the last op took on each stream.

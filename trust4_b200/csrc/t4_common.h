@@ -21,6 +21,7 @@ typedef int64_t i64;
 #define T4_HD __host__ __device__
 #define T4_D __device__
 #define T4_SYNC() __syncthreads()
+#define T4_SYNC_OR( x ) __syncthreads_or( x )
 // Large collective routines with several call sites are real functions in the product build: inlined everywhere the
 // stream kernel was 70 k SASS instructions (1.1 MB) and 18 % of its stall cycles were instruction fetch.
 #ifdef T4_INLINE_ALL
@@ -34,6 +35,7 @@ typedef int64_t i64;
 #define T4_HD
 #define T4_D
 #define T4_SYNC() ((void)0)
+#define T4_SYNC_OR( x ) ( x )
 #endif
 
 #define T4_DEV_MAX_READ T4_MAX_READ_LEN       /* device-side read length limit (reads > 200 bp make the reference switch to isLongSeqSet) */
@@ -161,6 +163,108 @@ struct T4Pos               // per (strand pass, read position) lookup record
 	u32 base ;                     // first hit slot, 0xffffffff = lookup not taken
 } ;
 
+// ---- contigs out of the arena: block bodies of t4_gather_kernel, t4_pack_size_kernel and t4_pack_kernel ----
+// Contig c's payload into one contiguous buffer: [consensus len][posWeight 16*len][name nameLen] at out + outOff[c].
+T4_D inline void t4_gather_block( char *A, const T4Contig *ct, const u64 *outOff, char *out, int n, int c, u32 tid, u32 nt )
+{
+	if ( c >= n || ct[c].consOff == 0 )
+		return ;
+	const T4Contig &k = ct[c] ;
+	char *o = out + outOff[c] ;
+	const char *cons = A + k.consOff + k.lead ;
+	const char *pw = A + k.pwOff + 16ull * k.lead ;
+	const char *nm = A + k.nameOff ;
+	for ( int i = tid ; i < k.len ; i += nt )
+		o[i] = cons[i] ;
+	for ( int i = tid ; i < 16 * k.len ; i += nt )
+		o[k.len + i] = pw[i] ;
+	for ( int i = tid ; i < k.nameLen ; i += nt )
+		o[17 * k.len + i] = nm[i] ;
+}
+
+// Stream j: decide for every live contig whether its posWeight counts fit 16 bits (scratch flag in the contig record),
+// and sum the record sizes.
+T4_D inline void t4_pack_size_block( char *A, const u64 *streamOff, u64 *sizes, u64 *counts, u32 j, u32 tid, u32 nt )
+{
+	const T4Stream *st = (const T4Stream *)( A + streamOff[j] ) ;
+	T4Contig *ct = (T4Contig *)( A + st->seqsOff ) ;
+	u64 tot = 0, n = 0 ;
+	for ( int i = 0 ; i < st->nSeqs ; ++i )
+	{
+		T4Contig &k = ct[i] ;
+		if ( !k.consOff )
+			continue ;
+		const int *pw = (const int *)( A + k.pwOff + 16ull * k.lead ) ;
+		int wide = 0 ;
+		for ( int x = tid ; x < 4 * k.len ; x += nt )
+			wide |= ( (unsigned)pw[x] > 65535u ) ;
+		wide = T4_SYNC_OR( wide ) ;
+		if ( tid == 0 )
+			k.packNarrow = wide ? 0 : 1 ;
+		T4_SYNC() ;
+		tot += t4_pack_record_bytes( k ) ;
+		++n ;
+	}
+	if ( tid == 0 )
+	{
+		sizes[j] = tot ;
+		counts[j] = n ;
+	}
+}
+
+// Stream j's live contigs as packed records (t4_pack_record_bytes) from out + outOff[j] on.
+T4_D inline void t4_pack_block( char *A, const u64 *streamOff, const u64 *outOff, char *out, u32 j, u32 tid, u32 nt )
+{
+	const T4Stream *st = (const T4Stream *)( A + streamOff[j] ) ;
+	const T4Contig *ct = (const T4Contig *)( A + st->seqsOff ) ;
+	u64 o = outOff[j] ;
+	for ( int i = 0 ; i < st->nSeqs ; ++i )
+	{
+		const T4Contig &k = ct[i] ;
+		if ( !k.consOff )
+			continue ;
+		u64 rb = t4_pack_record_bytes( k ) ;
+		char *rec = out + o ;
+		if ( tid == 0 )
+		{
+			u32 *h = (u32 *)rec ;
+			h[0] = j ; h[1] = (u32)i ; h[2] = (u32)k.len ; h[3] = (u32)k.nameLen ;
+			h[4] = (u32)k.barcode ; h[5] = (u32)k.numRead ; h[6] = (u32)rb ; h[7] = k.packNarrow ? 1u : 0u ;
+		}
+		const char *cons = A + k.consOff + k.lead ;
+		const int *pw = (const int *)( A + k.pwOff + 16ull * k.lead ) ;
+		const char *nm = A + k.nameOff ;
+		for ( int x = tid ; x < k.len ; x += nt )
+			rec[32 + x] = cons[x] ;
+		u64 nameAt ;
+		if ( k.packNarrow )
+		{
+			// the columns start at byte 32 + len (any alignment): byte stores
+			unsigned char *d = (unsigned char *)rec + 32 + k.len ;
+			for ( int x = tid ; x < 4 * k.len ; x += nt )
+			{
+				const unsigned v = (unsigned)pw[x] ;
+				d[2 * x] = (unsigned char)( v & 255u ) ;
+				d[2 * x + 1] = (unsigned char)( v >> 8 ) ;
+			}
+			nameAt = 32ull + 9ull * k.len ;
+		}
+		else
+		{
+			const char *pb = (const char *)pw ;
+			for ( int x = tid ; x < 16 * k.len ; x += nt )
+				rec[32 + k.len + x] = pb[x] ;
+			nameAt = 32ull + 17ull * k.len ;
+		}
+		for ( int x = tid ; x < k.nameLen ; x += nt )
+			rec[nameAt + x] = nm[x] ;
+		// tail padding of the 16-byte aligned record: defined bytes (the all-gathered buffers are compared bytewise)
+		for ( u64 x = nameAt + k.nameLen + tid ; x < rb ; x += nt )
+			rec[x] = 0 ;
+		o += rb ;
+	}
+}
+
 // ---- 2-bit packed reads (KmerCode.hpp:94-109 semantics on words) ----
 // A read of `len` bases occupies t4_pack_words(len) u64 words, W = ceil(len / 32):
 //   fw[W]  forward strand, base j in bits [63 - 2 (j & 31) - 1, 63 - 2 (j & 31)] of word j >> 5 (first base most
@@ -199,6 +303,38 @@ T4_HD inline void t4_pack_word( const char *s, int len, int w, u64 *fw, u64 *rc,
 	*fw = f ;
 	*rc = b ;
 	*nm = mk ;
+}
+
+// ASCII pool -> 2-bit packed pool (t4_pack_reads_kernel): item g = word g % wMax of read g / wMax.  *odd is set when a
+// read holds a character outside ACGTN (the packed form cannot represent it; callers then keep using the ASCII pool).
+struct T4PackReadsParams
+{
+	const t4_read_desc *descs ;
+	i64 n ;
+	const char *pool ;
+	u64 packStride ;               // u64 words per record
+	int wMax ;                     // words of the longest read
+	u64 *packed ;
+	u32 *odd ;
+} ;
+
+T4_HD inline void t4_pack_read_word( const T4PackReadsParams &P, i64 g )
+{
+	const i64 r = g / P.wMax ;
+	const int w = (int)( g % P.wMax ) ;
+	if ( r >= P.n )
+		return ;
+	const int len = P.descs[r].len ;
+	if ( len <= 0 || len > T4_DEV_MAX_READ )
+		return ;
+	const int W = (int)t4_pack_w( len ) ;
+	if ( w >= W )
+		return ;
+	u64 *fw = P.packed + (u64)r * P.packStride, *rc = fw + W ;
+	u32 *nm = (u32 *)( fw + 2 * W ) ;
+	t4_pack_word( P.pool + P.descs[r].seq_off, len, w, fw + w, rc + w, nm + w, P.odd ) ;
+	if ( w == 0 && ( W & 1 ) )
+		nm[W] = 0 ;
 }
 
 // Pointers to buffers outside the arena (workloads, staging, outputs) are absolute addresses stored in u64.

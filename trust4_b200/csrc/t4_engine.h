@@ -73,6 +73,20 @@ struct T4Ctx
 	template <class T> T4_HD T *P( u64 off ) const { return (T *)( A + off ) ; }
 } ;
 
+// The context of thread tid of nt working on the stream at arena offset streamOff.
+T4_HD inline T4Ctx t4_ctx( char *A, u64 streamOff, T4Smem *sm, int tid, int nt )
+{
+	T4Ctx cx ;
+	cx.A = A ;
+	cx.g = (T4Global *)A ;
+	cx.st = (T4Stream *)( A + streamOff ) ;
+	cx.sm = sm ;
+	cx.cap = cx.g->cap ;
+	cx.tid = tid ;
+	cx.nt = nt ;
+	return cx ;
+}
+
 #define T4_PAR_FOR( i, n ) for ( int i = cx.tid ; i < (int)( n ) ; i += cx.nt )
 
 T4_D inline u64 t4_atomic_cas( u64 *p, u64 cmp, u64 val ) ;
@@ -1205,6 +1219,33 @@ T4_HD inline int t4_dp_posweight( const int *tw, int lent, const char *p, int le
 		align[j] = tmp ;
 	}
 	return ret ;
+}
+
+// n independent GlobalAlignment_PosWeight problems (t4_dp_kernel): problem i aligns p[pOff[i] .. pOff[i + 1]) to the
+// columns tw[4 tOff[i] .. 4 tOff[i + 1]) into align + alignOff[i], with its rows and traceback at scratch + scratchOff[i].
+struct T4DpParams
+{
+	const int *tw ;
+	const i64 *tOff ;
+	const char *p ;
+	const i64 *pOff ;
+	signed char *align ;
+	const i64 *alignOff ;
+	int *score ;
+	char *scratch ;
+	const i64 *scratchOff ;
+	int n ;
+} ;
+
+T4_HD inline void t4_dp_one( const T4DpParams &P, i64 i )
+{
+	int lent = (int)( P.tOff[i + 1] - P.tOff[i] ) ;
+	int lenp = (int)( P.pOff[i + 1] - P.pOff[i] ) ;
+	int d = lent > lenp ? lent - lenp : lenp - lent ;
+	int W = 2 * T4_DP_BAND + 3 + d ;
+	char *s = P.scratch + P.scratchOff[i] ;
+	P.score[i] = t4_dp_posweight( P.tw + 4 * P.tOff[i], lent, P.p + P.pOff[i], lenp, P.align + P.alignOff[i], (int *)s,
+		(unsigned char *)( s + 8 * W ), 0 ) ;
 }
 
 // The same alignment for lent == lenp == n (every hot-path call: overhangs and same-diagonal gaps), band +-5.
@@ -3439,57 +3480,6 @@ T4_D T4_BIG int c_add_read( T4Ctx &cx, int len, const char *geneName, int &stran
 		T4_SYNC() ;
 		if ( !easy )
 		{
-#if T4_CUDA && defined( T4_EXT_WARP_DP )
-			// Variant (off): one warp per overlap, the left overhang's DP on lanes 0..15, the right one's on lanes 16..31, both
-			// on the anti-diagonal schedule of w_dp_equal_half (2 n + 12 shuffle steps instead of 13 n cells walked by one
-			// thread).  Parity green, but measured equal to the thread-per-side form below (606.5 vs 609.5 ms per launch on the
-			// bench workload): a step costs two dependent shuffles, a row of the register-resident DP about as much, and the
-			// thread form runs all sides of a read at once instead of four overlaps at a time.
-			{
-				T4Smem *sm = cx.sm ;
-				const int warp = cx.tid >> 5, nwarps = cx.nt >> 5, lane = cx.tid & 31, half = lane >> 4 ;
-				for ( int i = warp ; i < overlapCnt ; i += nwarps )
-				{
-					const bool dl = sstats[2 * i].ind == -1, dr = sstats[2 * i + 1].ind == -1 ;
-					if ( !dl && !dr )
-						continue ;
-					const T4Ovl o = overlaps[i] ;
-					T4Contig *seq = t4_seq( cx, o.seqIdx ) ;
-					const int *pw = t4_pw( cx, seq ) ;
-					const int L = t4_min( o.readStart, o.seqStart ), R = t4_min( len - 1 - o.readEnd, seq->len - 1 - o.seqEnd ) ;
-					const char *pl = r + o.readStart - L, *pr = r + o.readEnd + 1 ;
-					if ( dl )
-						w_stage_side( pw + 4 * ( o.seqStart - L ), pl, L, sm->wnib[warp][0], sm->wbits[warp][0], lane ) ;
-					if ( dr )
-						w_stage_side( pw + 4 * ( o.seqEnd + 1 ), pr, R, sm->wnib[warp][1], sm->wbits[warp][1], lane ) ;
-					const int n = half ? ( dr ? R : 0 ) : ( dl ? L : 0 ) ;
-					const bool small = n < 16 * T4_WACT_WORDS ;
-					u32 *actBase = small ? sm->wact[warp][half] : (u32 *)t4_dp_scratch_of( cx, cx.tid & ~15 ).act ;
-					const int actStride = small ? T4_WACT_WORDS : (int)( T4_DP_STRIDE / 4 ) ;
-					signed char *abuf = small ? sm->wal[warp][half] : t4_align_of_thread( cx, cx.tid & ~15 ) ;
-					const int acap = small ? (int)sizeof( sm->wal[0][0] ) : 2 * T4_DEV_MAX_READ + 8 ;
-					int alen = 0 ;
-					w_dp_equal_half( cx, sm->wnib[warp][half], half ? pr : pl, n, abuf, acap, &alen, actBase, actStride ) ;
-					for ( int side = 0 ; side < 2 ; ++side )
-					{
-						if ( !( side ? dr : dl ) )
-							continue ;
-						T4AlignView v ;
-						v.n = __shfl_sync( T4_FULL, alen, 16 * side ) ;
-						v.a = (const signed char *)__shfl_sync( T4_FULL, (unsigned long long)( abuf + acap - 1 ), 16 * side ) - v.n ;
-						v.bits = 0 ;
-						v.dp = 1 ;
-						const T4SideStats ss = w_side_stats( v, side == 0, lane ) ;
-						if ( lane == 0 )
-						{
-							sstats[2 * i + side] = ss ;
-							t4_count( cx, 1, 1 ) ;
-						}
-					}
-					__syncwarp() ;
-				}
-			}
-#else
 			T4DpScratch ds = t4_dp_scratch( cx ) ;
 			T4_PAR_FOR( x, 2 * overlapCnt )
 			{
@@ -3514,7 +3504,6 @@ T4_D T4_BIG int c_add_read( T4Ctx &cx, int len, const char *geneName, int &stran
 					t4_count( cx, 1, 1 ) ;
 				sstats[x] = t4_side_stats( av, !right ) ;
 			}
-#endif
 			T4_SYNC() ;
 			T4_PAR_FOR( i, overlapCnt )
 			{
@@ -4648,6 +4637,13 @@ T4_D inline void c_init_stream( T4Ctx &cx, u64 base, const T4InitParams &ip )
 		dir[i].cnt = dir[i].cap = dir[i].lock = dir[i].pad = 0 ;
 	}
 	T4_SYNC() ;
+}
+
+// t4_init_kernel: block b lays out the b-th stream from base on, ip.footprint bytes apart
+T4_D inline void c_init_block( char *A, u64 base, const T4InitParams &ip, u32 b, int tid, int nt )
+{
+	T4Ctx cx = t4_ctx( A, 0, 0, tid, nt ) ;
+	c_init_stream( cx, base + (u64)b * ip.footprint, ip ) ;
 }
 
 // ---------------------------------------------------------------------------

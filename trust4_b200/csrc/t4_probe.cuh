@@ -657,30 +657,6 @@ __global__ void __launch_bounds__( 32 * T4P_WARPS, MINB ) t4_probe_kernel( T4Pro
 	}
 }
 
-// ASCII pool -> 2-bit packed pool (t4_common.h layout).  One thread per (read, word): 32 forward bases, 32
-// reverse-complement bases and 32 mask bits.  *odd is set when a read holds a character outside ACGTN (the packed
-// form cannot represent it; callers then keep using the ASCII pool for the assembly).
-__global__ void t4_pack_reads_kernel( const t4_read_desc *descs, i64 n, const char *pool, u64 packStride, int wMax, u64 *packed, u32 *odd )
-{
-	const i64 g = (i64)blockIdx.x * blockDim.x + threadIdx.x ;
-	const i64 r = g / wMax ;
-	const int w = (int)( g % wMax ) ;
-	if ( r >= n )
-		return ;
-	const int len = descs[r].len ;
-	if ( len <= 0 || len > T4_DEV_MAX_READ )
-		return ;
-	const int W = (int)t4_pack_w( len ) ;
-	if ( w >= W )
-		return ;
-	const char *s = pool + descs[r].seq_off ;
-	u64 *fw = packed + (u64)r * packStride, *rc = fw + W ;
-	u32 *nm = (u32 *)( fw + 2 * W ) ;
-	t4_pack_word( s, len, w, fw + w, rc + w, nm + w, odd ) ;
-	if ( w == 0 && ( W & 1 ) )
-		nm[W] = 0 ;
-}
-
 // Visit order of the probe: reads of one set together, inside a set by length bucket (32 bases per bucket, longest
 // first) so that the warps of a CTA carry equal numbers of k-mers.  One CTA per set.
 __global__ void t4_bucket_kernel( const t4_read_desc *descs, const i64 *descOff, u64 *ord )
