@@ -371,28 +371,28 @@ int t4_refset_scan(t4_refset *r, const char *read_pool, size_t pool_bytes, const
 /* SeqSet::GetOverlapsFromRead(read, 0, -1, 0, false, overlaps) on the gene set -- the call SeqSet::AnnotateRead makes per
  * read (SeqSet.hpp:6050), first half of the rough annotation (SURVEY.md 8f-1): chains with the reference-sequence rules
  * (or the V-end / J-start rescue, GetVJOverlapsFromHits), gaps scored by the affine AlignAlgo::GlobalAlignment, indels
- * allowed, similarity >= 0.75.  Same output layout as t4_seqset_get_overlaps.  Verified through the test emulation only
- * so far (no GPU run yet). */
+ * allowed, similarity >= 0.75.  Same output layout as t4_seqset_get_overlaps.  Verified on an H100 against the reference.
+ * A read with more seed hits than the per-read work space (65 536) returns T4_E_NOMEM; later calls are not affected. */
 int t4_refset_get_overlaps(t4_refset *r, const char *read, int32_t *overlaps, double *similarity, int cap);
 /* SeqSet::AnnotateRead(read, 0, geneOverlap, NULL, NULL) for n reads -- the rough annotation of the stage-1 driver
  * (main.cpp:1084-1120; SeqSet.hpp:6016-6340, detailLevel 0): contig intervals of the read (runs of N's), the overlaps of
  * every interval (above), the best gene per type with similarity >= 0.8, one cell type and chain per read, the check for a
  * random short constant-gene match.  gene_overlaps[i][t][8] for t = V, D, J, C = {seqIdx (-1: none), readStart, readEnd,
- * seqStart, seqEnd, strand, matchCnt, indelCnt}; similarity[i][t].  Host buffers.  Verified through the test emulation
- * only so far (no GPU run yet). */
+ * seqStart, seqEnd, strand, matchCnt, indelCnt}; similarity[i][t].  Host buffers.  Verified on an H100 against the
+ * reference.  A batch with a read over the per-read hit limit returns T4_E_NOMEM as a whole; later calls are not affected. */
 int t4_refset_annotate(t4_refset *r, const char *read_pool, size_t pool_bytes, const uint64_t *seq_off, const int32_t *len,
                        int64_t n, int32_t *gene_overlaps, double *similarity);
 /* std::sort(sortedReads.begin(), sortedReads.end()) of the stage-1 driver (main.cpp:1078) with _sortRead::operator<
  * (main.cpp:103-125: minCnt, medianCnt, avgCnt, length descending, then read string and id ascending): order[j] = index of
  * the j-th record.  Host buffers; ids are id_pool[id_off[i] .. id_off[i+1]).  A merge sort of independent binary searches
- * on the device.  Verified through the test emulation only so far (no GPU run yet). */
+ * on the device.  Verified on an H100 against the reference. */
 int t4_sort_reads(const char *read_pool, size_t pool_bytes, const uint64_t *seq_off, const int32_t *len, const char *id_pool,
                   size_t id_pool_bytes, const uint64_t *id_off, const int32_t *min_cnt, const int32_t *median_cnt,
                   const float *avg_cnt, int64_t n, int64_t *order);
 /* AlignAlgo::IsMateOverlap(fr, flen, sr, slen, minOverlap, offset, bestMatchCnt, checkTandem) (AlignAlgo.hpp:1027-1096)
  * for n read pairs, as ProcessRead calls it to detect read-through and overlapping mates (main.cpp:264, 291): overlap_size[i]
  * is the return value (-1: no unambiguous overlap), offset[i] / best_match_cnt[i] the two outputs as the function leaves them
- * (-1 when it never assigned them).  Host buffers.  Verified through the test emulation only so far (no GPU run yet). */
+ * (-1 when it never assigned them).  Host buffers.  Verified on an H100 against the reference. */
 int t4_mate_overlap_batch(const char *read_pool, size_t pool_bytes, const uint64_t *f_off, const int32_t *f_len,
                           const uint64_t *s_off, const int32_t *s_len, const int32_t *min_overlap,
                           const uint8_t *check_tandem, int64_t n, int32_t *overlap_size, int32_t *offset,

@@ -988,21 +988,11 @@ def check_refset_overlaps(lib, ref, tmp_path, seed=131, n=500, radius=None, hit_
     return n_ovl
 
 
-def check_refset_annotate(lib, ref, tmp_path, seed=141, n=600, radius=None, hit_len=31, k=9):
-    """t4_refset_annotate against SeqSet::AnnotateRead(read, 0, geneOverlap, NULL, NULL) -- the rough annotation the stage-1
-    driver runs on every read (main.cpp:1084-1120): per gene type V / D / J / C the chosen gene, coordinates, strand, matchCnt,
-    indelCnt, similarity.  Reads: clonotype reads (V + junction + J + C in one read), mutated gene pieces, V/J-only ends,
+def annotate_reads(recs, n, seed):
+    """Reads for the rough annotation: clonotype reads (V + junction + J + C in one read), mutated gene pieces, V/J-only ends,
     reverse strands, chimeras of two chains (one chain per read rule), random reads, reads cut into several contigs by runs
-    of N's, short constant-gene matches."""
+    of N's, short constant-gene matches.  recs: the (name, sequence) list write_gene_fasta returns."""
     rng = np.random.default_rng(seed)
-    fa = os.path.join(str(tmp_path), "genes_a%d.fa" % seed)
-    recs = write_gene_fasta(fa)
-    lib.check(lib.reset())
-    g = api.RefSet(fa, k, lib, hit_len_required=hit_len)
-    r = ref.RefGeneSet(fa, k, hit_len_required=hit_len)
-    if radius is not None:
-        g.set_radius(radius)
-        r.set_radius(radius)
     cl = synth.make_clones(60, seed)
     rd = synth.sample_pairs(cl, n // 3, 150, seed, sub_rate=0.02)
     reads = [synth.decode(c) for c in rd.codes]
@@ -1044,21 +1034,52 @@ def check_refset_annotate(lib, ref, tmp_path, seed=141, n=600, radius=None, hit_
         else:
             t = base[: int(rng.integers(30, 100))]
         reads.append(t[:400])
-    lens = np.array([len(x) for x in reads], dtype=np.int32)
-    off = np.zeros(len(reads), dtype=np.uint64)
-    off[1:] = np.cumsum(lens[:-1])
-    pool = np.frombuffer(("".join(reads) + "\0" * 16).encode(), dtype=np.uint8).copy()
-    go, gsim = g.annotate(pool, off, lens)
+    return reads[:n]
+
+
+def reads_pool(reads):
+    """(pool, seq_off, lens) of a list of str / bytes reads laid end to end."""
+    rb = [x if isinstance(x, bytes) else x.encode() for x in reads]
+    lens = np.array([len(x) for x in rb], dtype=np.int32)
+    off = np.zeros(len(rb), dtype=np.uint64)
+    if len(rb) > 1:
+        off[1:] = np.cumsum(lens[:-1])
+    pool = np.frombuffer(b"".join(rb) + b"\0" * 16, dtype=np.uint8).copy()
+    return pool, off, lens
+
+
+def compare_annotations(go, gsim, reads, ann, tag=""):
+    """t4_refset_annotate's output for `reads` against the reference's AnnotateRead results `ann` (one (int32[4, 8],
+    similarity[4]) pair per read); returns how many gene entries per type V, D, J, C are set."""
+    assert len(go) == len(reads) == len(ann), (tag, len(go), len(reads), len(ann))
     n_set = np.zeros(4, dtype=np.int64)
     for i, t in enumerate(reads):
-        ro, rsim = r.annotate_read(t)
-        assert (go[i][:, 0] == ro[:, 0]).all(), ("gene", i, go[i][:, 0], ro[:, 0], t)
+        ro, rsim = ann[i]
+        assert (go[i][:, 0] == ro[:, 0]).all(), ("gene", tag, i, go[i][:, 0], ro[:, 0], t)
         for tt in range(4):
             if ro[tt, 0] >= 0:
-                assert (go[i][tt] == ro[tt]).all() and gsim[i][tt] == rsim[tt], ("overlap", i, tt, go[i][tt], ro[tt], gsim[i][tt], rsim[tt], t)
+                assert (go[i][tt] == ro[tt]).all() and gsim[i][tt] == rsim[tt], ("overlap", tag, i, tt, go[i][tt], ro[tt], gsim[i][tt], rsim[tt], t)
                 n_set[tt] += 1
             else:
-                assert go[i][tt][5] == 1       # strand of an unset entry
+                assert go[i][tt][5] == 1, (tag, i)       # strand of an unset entry
+    return n_set
+
+
+def check_refset_annotate(lib, ref, tmp_path, seed=141, n=600, radius=None, hit_len=31, k=9):
+    """t4_refset_annotate against SeqSet::AnnotateRead(read, 0, geneOverlap, NULL, NULL) -- the rough annotation the stage-1
+    driver runs on every read (main.cpp:1084-1120): per gene type V / D / J / C the chosen gene, coordinates, strand, matchCnt,
+    indelCnt, similarity.  Reads: see annotate_reads."""
+    fa = os.path.join(str(tmp_path), "genes_a%d.fa" % seed)
+    recs = write_gene_fasta(fa)
+    lib.check(lib.reset())
+    g = api.RefSet(fa, k, lib, hit_len_required=hit_len)
+    r = ref.RefGeneSet(fa, k, hit_len_required=hit_len)
+    if radius is not None:
+        g.set_radius(radius)
+        r.set_radius(radius)
+    reads = annotate_reads(recs, n, seed)
+    go, gsim = g.annotate(*reads_pool(reads))
+    n_set = compare_annotations(go, gsim, reads, [r.annotate_read(t) for t in reads])
     assert n_set[0] > n // 5 and n_set[2] > n // 20 and n_set[3] > n // 10, n_set
     g.close()
     return int(n_set.sum())
@@ -1175,3 +1196,426 @@ def check_mate_overlap(lib, ref, seed=161, n=3000):
         n_pos += r >= 0
     assert n_pos > n // 5 and n_pos < n
     return n_pos
+
+
+def check_sort_reads_tiny(lib, ref):
+    """t4_sort_reads on 0 .. 3 records (no pass, one pass, a ragged last run)."""
+    pool = np.frombuffer(b"ACGTACGTAC" + b"\0" * 16, dtype=np.uint8).copy()
+    for n in (0, 1, 2, 3):
+        ids = ["r%d" % (9 - i) for i in range(n)]
+        order = api.sort_reads(pool, np.arange(n, dtype=np.uint64), np.full(n, 5, dtype=np.int32), ids,
+                               np.ones(n, np.int32), np.ones(n, np.int32), np.ones(n, np.float32), lib)
+        reads = [bytes(pool[i:i + 5]).decode() for i in range(n)]
+        assert order.tolist() == ref.sort_reads(reads, ids, np.ones(n), np.ones(n), np.ones(n)).tolist()
+
+
+def sort_key(reads, ids, mn, med, avg):
+    """_sortRead::operator< (main.cpp:103-125) as a Python key: counts and length descending, then the read and the id as
+    bytes -- Python orders bytes like strcmp on unsigned char, the shorter string first on a common prefix.  -0.0 and 0.0
+    are equal keys, as they are equal floats in the comparator."""
+    return lambda i: (-int(mn[i]), -int(med[i]), -float(avg[i]), -len(reads[i]), reads[i], ids[i])
+
+
+def _check_sorted_records(go, keys, want):
+    """go (the library's order) holds every index once and lists the same records as `want`; records equal in every field
+    may come in either order, so the records are compared, not the indices."""
+    n = len(keys)
+    assert len(go) == n and (np.sort(go) == np.arange(n)).all(), "not a permutation"
+    bad = [j for j, (a, b) in enumerate(zip(go, want)) if keys[a] != keys[b]]
+    assert not bad, ("order", bad[:5], [keys[go[j]][:4] for j in bad[:2]], [keys[want[j]][:4] for j in bad[:2]])
+
+
+def _ref_sort_bytes(ref, reads, ids, mn, med, avg):
+    """The reference's std::sort on byte strings (bytes >= 0x80 included)."""
+    import ctypes as C
+    n = len(reads)
+    ra = (C.c_char_p * max(1, n))(*reads)
+    ia = (C.c_char_p * max(1, n))(*ids)
+    order = np.zeros(max(1, n), dtype=np.int64)
+    ref.lib().t4ref_sort_reads(ra, ia, np.ascontiguousarray(mn, dtype=np.int32).ctypes.data, np.ascontiguousarray(med, dtype=np.int32).ctypes.data,
+                               np.ascontiguousarray(avg, dtype=np.float32).ctypes.data, n, order.ctypes.data)
+    return order[:n]
+
+
+def check_sort_reads_large(lib, seed=153, n=(1 << 20) + 3):
+    """t4_sort_reads at a size where the sort kernel's grid-stride loop turns more than once (n above the launch cap, a ragged
+    last run): synthetic read pairs with their real 21-mer statistics (t4_kmer_count_stats), lengths cut at random, half
+    of the statistics coarsened so that long runs of ties are decided by the read strings and then the ids -- against the
+    plain Python restatement of the comparator (sort_key)."""
+    rng = np.random.default_rng(seed)
+    cl = synth.make_clones(200, seed)
+    rd = synth.sample_pairs(cl, (n + 1) // 2, 150, seed, sub_rate=0.01)
+    L = rd.codes.shape[1]
+    pool = np.concatenate([np.frombuffer(b"ACGT", dtype=np.uint8)[rd.codes[:n]].reshape(-1), np.zeros(16, dtype=np.uint8)])
+    off = (np.arange(n, dtype=np.uint64) * np.uint64(L))
+    lens = np.where(rng.random(n) < 0.3, rng.integers(20, L + 1, size=n), L).astype(np.int32)
+    ids = [b"r%d" % (i // 2) + (b".1" if x < 0.1 else b"") for i, x in zip(range(n), rng.random(n))]
+    mn, med, avg, _ = api.kmer_count_stats(pool, off, lens, 21, lib)
+    coarse = rng.random(n) < 0.5
+    mn = np.where(coarse, np.minimum(mn, 2), mn).astype(np.int32)
+    med = np.where(coarse, np.minimum(med, 3), med).astype(np.int32)
+    avg = np.where(coarse, np.float32(2.5), avg).astype(np.float32)
+    go = api.sort_reads(pool, off, lens, ids, mn, med, avg, lib)
+    pb = pool.tobytes()
+    reads = [pb[o:o + l] for o, l in zip(off.tolist(), lens.tolist())]
+    key = sort_key(reads, ids, mn.tolist(), med.tolist(), avg.tolist())
+    keys = [key(i) for i in range(n)]
+    want = sorted(range(n), key=keys.__getitem__)
+    _check_sorted_records(go, keys, want)
+    ties = sum(1 for a, b in zip(want, want[1:]) if keys[a][:4] == keys[b][:4])
+    assert ties > n // 4, ties       # the strings really decide a large part of the order
+    return n
+
+
+def sort_edge_records(seed, n_base=1500):
+    """Records for the comparator's edges: (reads, ids, min, median, avg).  Few distinct counts (long ties); reads and ids
+    that differ first at a byte >= 0x80 against one < 0x80; reads longer than 512 bp that differ only late; avg values one
+    float ulp apart, -0.0 next to 0.0; negative counts; groups of records equal in every field, scattered over the array so
+    that equal records meet in different runs of every merge pass."""
+    rng = np.random.default_rng(seed)
+    avgs = [np.float32(1.0), np.nextafter(np.float32(1.0), np.float32(2)), np.nextafter(np.float32(1.0), np.float32(0)),
+            np.float32(0.0), np.float32(-0.0), np.float32(2.5), np.float32(-1.5)]
+
+    def rnd(L):
+        return bytes(rng.choice(np.frombuffer(b"ACGT", dtype=np.uint8), size=L))
+
+    recs = []
+
+    def stats():
+        return int(rng.choice([-1, 0, 1, 2])), int(rng.choice([0, 1, 3])), avgs[int(rng.integers(len(avgs)))]
+
+    for i in range(n_base):
+        kind = int(rng.integers(0, 6))
+        mn, med, av = stats()
+        if kind == 0:                      # a high byte against a low one at the same position, same counts and length
+            r = bytearray(rnd(int(rng.integers(10, 40))))
+            p = int(rng.integers(len(r)))
+            r2 = bytearray(r)
+            r[p] = int(rng.integers(0x80, 0x100))
+            r2[p] = int(rng.integers(0x41, 0x80))
+            recs.append((bytes(r), b"h%d" % i, mn, med, av))
+            recs.append((bytes(r2), b"h%d" % i, mn, med, av))
+        elif kind == 1:                    # same read, ids that differ at a high byte / are prefixes of each other
+            r = rnd(int(rng.integers(10, 40)))
+            for idb in (b"id\xe9", b"id\x7f", b"id", b"id\xff\x01", b"id\x80"):
+                recs.append((r, idb, mn, med, av))
+        elif kind == 2:                    # longer than 512 bp, differing only after position 512 (or a prefix)
+            base = rnd(int(rng.integers(513, 1001)))
+            q = int(rng.integers(512, len(base)))
+            other = base[:q] + (b"A" if base[q:q + 1] != b"A" else b"C") + base[q + 1:]
+            recs.append((base, b"l%d" % i, mn, med, av))
+            recs.append((other, b"l%d" % i, mn, med, av))
+            recs.append((base[:q], b"l%d" % i, mn, med, av))
+        elif kind == 3:                    # avg one ulp apart, -0.0 next to 0.0, everything else equal
+            r = rnd(int(rng.integers(10, 40)))
+            for av2 in avgs:
+                recs.append((r, b"u%d" % i, mn, med, av2))
+        elif kind == 4:                    # a group of records equal in every field
+            rec = (rnd(int(rng.integers(5, 30))), b"e%d" % (i % 7), mn, med, av)
+            recs.extend([rec] * int(rng.choice([2, 3, 5, 17, 40])))
+        else:
+            recs.append((rnd(int(rng.integers(5, 60))), b"r%d" % int(rng.integers(0, 50)), mn, med, av))
+    perm = rng.permutation(len(recs))
+    recs = [recs[int(j)] for j in perm]
+    reads = [x[0] for x in recs]
+    ids = [x[1] for x in recs]
+    mn = np.array([x[2] for x in recs], dtype=np.int32)
+    med = np.array([x[3] for x in recs], dtype=np.int32)
+    avg = np.array([x[4] for x in recs], dtype=np.float32)
+    return reads, ids, mn, med, avg
+
+
+def check_sort_reads_edges(lib, ref, seed=154, n_base=1500):
+    """t4_sort_reads at the comparator's edges (sort_edge_records), against the reference's std::sort and the Python key."""
+    reads, ids, mn, med, avg = sort_edge_records(seed, n_base)
+    pool, off, lens = reads_pool(reads)
+    go = api.sort_reads(pool, off, lens, ids, mn, med, avg, lib)
+    key = sort_key(reads, ids, mn.tolist(), med.tolist(), avg.tolist())
+    keys = [key(i) for i in range(len(reads))]
+    _check_sorted_records(go, keys, _ref_sort_bytes(ref, reads, ids, mn, med, avg))
+    _check_sorted_records(go, keys, sorted(range(len(reads)), key=keys.__getitem__))
+    assert max(lens) > 512 and any(b >= 0x80 for r in reads for b in r)
+    return len(reads)
+
+
+def _mate_batch(lib, fr, sr, mo, ct):
+    """t4_mate_overlap_batch over the pairs (fr[i], sr[i]) (str or bytes): (overlap_size, offset, best_match_cnt)."""
+    n = len(fr)
+    pool, off, lens = reads_pool(list(fr) + list(sr))
+    fo, so = off[:n].copy(), off[n:].copy()
+    fl, sl = lens[:n].copy(), lens[n:].copy()
+    mo = np.ascontiguousarray(mo, dtype=np.int32)
+    ct = np.ascontiguousarray(ct, dtype=np.uint8)
+    gos, gof, gbm = (np.zeros(max(1, n), dtype=np.int32) for _ in range(3))
+    lib.check(lib.mate_overlap_batch(pool.ctypes.data, pool.nbytes, fo.ctypes.data, fl.ctypes.data, so.ctypes.data, sl.ctypes.data,
+                                     mo.ctypes.data, ct.ctypes.data, n, gos.ctypes.data, gof.ctypes.data, gbm.ctypes.data))
+    return gos[:n], gof[:n], gbm[:n]
+
+
+def _mate_ref_check(ref, fr, sr, mo, ct, got):
+    """Every pair against AlignAlgo::IsMateOverlap of the reference; returns the return values."""
+    import ctypes as C
+    l = ref.lib()
+    gos, gof, gbm = got
+    out = np.zeros(len(fr), dtype=np.int32)
+    o, b = C.c_int32(), C.c_int32()
+    for i in range(len(fr)):
+        f = fr[i] if isinstance(fr[i], bytes) else fr[i].encode()
+        s = sr[i] if isinstance(sr[i], bytes) else sr[i].encode()
+        r = l.t4ref_is_mate_overlap(f, len(f), s, len(s), int(mo[i]), int(ct[i]), C.byref(o), C.byref(b))
+        assert (r, o.value, b.value) == (int(gos[i]), int(gof[i]), int(gbm[i])), (i, r, o.value, b.value, gos[i], gof[i], gbm[i], f, s, int(mo[i]), int(ct[i]))
+        out[i] = r
+    return out
+
+
+def _mate_threshold_count(L):
+    """int(L * similarityThreshold) of IsMateOverlap for an overlap of L bases (AlignAlgo.hpp:1042-1047)."""
+    t = 0.95
+    if L >= 100:
+        t = 0.85
+    elif L >= 50:
+        t = 0.85 + (L - 50) / 50.0 * 0.1
+    return int(L * t)
+
+
+def mate_edge_pairs(seed, reps=6):
+    """Pairs at the edges of IsMateOverlap: (fr, sr, minOverlap, checkTandem, tag) lists.
+    - zero-length mates; minOverlap >= flen; minOverlap = 0;
+    - mates up to 1000 bp whose only overlap has L = 49, 50, 51, 99, 100, 101 (the 0.95 / sloped / 0.85 threshold steps) or
+      more bases, with exactly as many mismatches as the threshold allows, one fewer and one more;
+    - N's and lower-case bases (compared as plain characters);
+    - an overlap of exactly 2 x minOverlap that is a tandem repeat (w + w, |w| = minOverlap), and the same one base longer."""
+    rng = np.random.default_rng(seed)
+    comp = {"A": "C", "C": "G", "G": "T", "T": "A"}
+
+    def rnd(L):
+        return "".join("ACGT"[c] for c in rng.integers(0, 4, size=L))
+
+    fr, sr, mo, ct, tag = [], [], [], [], []
+
+    def add(f, s, m, c, t):
+        fr.append(f); sr.append(s); mo.append(m); ct.append(c); tag.append(t)
+
+    for c in (0, 1):
+        add("", "", 0, c, "empty")
+        add("", rnd(50), 5, c, "empty f")
+        add(rnd(50), "", 5, c, "empty s")
+        add("", "", 3, c, "empty")
+    for _ in range(reps):
+        for c in (0, 1):
+            f = rnd(int(rng.integers(1, 60)))
+            add(f, f, len(f), c, "minOverlap = flen")
+            add(f, f, len(f) + int(rng.integers(1, 20)), c, "minOverlap > flen")
+            g = rnd(int(rng.integers(20, 120)))
+            q = int(rng.integers(1, len(g)))
+            add(g, g[len(g) - q:] + rnd(int(rng.integers(0, 30))), 0, c, "minOverlap 0")
+            add(g, rnd(int(rng.integers(0, 80))), 0, c, "minOverlap 0, random")
+    for L in (49, 50, 51, 99, 100, 101, 150, 400, 1000):
+        need = _mate_threshold_count(L)
+        for extra in (-1, 0, 1):
+            x = L - need + extra           # mismatches: need - 1 matches fail, need pass
+            if x < 0:
+                continue
+            for _ in range(reps):
+                flen = int(rng.integers(L, 1001))
+                f = rnd(flen)
+                ov = list(f[flen - L:])
+                for p in rng.choice(L, size=x, replace=False):
+                    ov[int(p)] = comp[ov[int(p)]]
+                s = "".join(ov) + rnd(int(rng.integers(0, 1001 - L)))
+                add(f, s, int(rng.integers(5, 32)), int(rng.integers(0, 2)), "threshold L=%d mismatches=%d" % (L, x))
+    for _ in range(8 * reps):
+        L = int(rng.integers(20, 160))
+        f = list(rnd(L + int(rng.integers(0, 60))))
+        j = len(f) - L
+        s = f[j:] + list(rnd(int(rng.integers(0, 60))))
+        for p in rng.integers(0, len(s), size=int(rng.integers(1, 6))):
+            s[int(p)] = "N" if rng.random() < 0.5 else s[int(p)].lower()
+        for p in rng.integers(0, len(f), size=int(rng.integers(0, 4))):
+            f[int(p)] = "N" if rng.random() < 0.5 else f[int(p)].lower()
+        add("".join(f), "".join(s), int(rng.integers(5, 20)), int(rng.integers(0, 2)), "N / lower case")
+    for m in (3, 5, 8, 12, 20, 31):
+        for _ in range(reps):
+            w = rnd(m)
+            for longer in (0, 1):
+                core = w + w + (rnd(1) if longer else "")
+                f = rnd(int(rng.integers(10, 80))) + core
+                s = core + rnd(int(rng.integers(0, 80)))
+                for c in (0, 1):
+                    add(f, s, m, c, "tandem 2 x minOverlap" + (" + 1" if longer else ""))
+    return fr, sr, mo, ct, tag
+
+
+def check_mate_overlap_edges(lib, ref, seed=163, reps=6):
+    """t4_mate_overlap_batch at the edges of IsMateOverlap (mate_edge_pairs) against the reference, pair by pair; the
+    threshold and tandem cases must really land on both sides."""
+    fr, sr, mo, ct, tag = mate_edge_pairs(seed, reps)
+    ret = _mate_ref_check(ref, fr, sr, mo, ct, _mate_batch(lib, fr, sr, mo, ct))
+    by = {}
+    for t, r in zip(tag, ret):
+        by.setdefault(t, []).append(int(r))
+    for L in (49, 50, 51, 99, 100, 101):
+        need = _mate_threshold_count(L)
+        assert all(r == -1 for r in by["threshold L=%d mismatches=%d" % (L, L - need + 1)]), L
+        assert sum(r == L for r in by["threshold L=%d mismatches=%d" % (L, L - need)]) >= len(by["threshold L=%d mismatches=%d" % (L, L - need)]) // 2, L
+    assert all(r == -1 for t, rs in by.items() if t.startswith("empty") or t.startswith("minOverlap >") for r in rs)
+    tandem = [r for t, rs in by.items() if t == "tandem 2 x minOverlap" for r in rs]
+    assert -1 in tandem and any(r > 0 for r in tandem)
+    return len(fr)
+
+
+def write_bad_gene_fasta(path):
+    """The bundled gene pool plus one gene of 2000 ACG repeats: a read of ACG repeats has far more seed hits on it than the
+    per-read scratch of the annotation holds (T4_E_NOMEM), while every other read is answered as usual."""
+    recs = write_gene_fasta(path)
+    s = "ACG" * 2000
+    with open(path, "a") as f:
+        f.write(">IGHV9-99*01\n")
+        for p in range(0, len(s), 60):
+            f.write(s[p:p + 60] + "\n")
+    return recs
+
+
+BAD_READ = "ACG" * 100
+
+
+def _expect_error(code, fn, *a):
+    try:
+        fn(*a)
+    except api.T4Error as e:
+        assert e.code == code, (e.code, code, str(e))
+        return
+    raise AssertionError("expected error %d" % code)
+
+
+def _check_overlaps_read(g, r, t):
+    gn, go, gsim = g.get_overlaps(t)
+    rn, ro, rsim = r.get_overlaps(t, 0, -1, False)
+    assert gn == rn, ("count", gn, rn, t)
+    if rn > 0:
+        assert (go == ro).all() and (gsim == rsim).all(), ("overlaps", t)
+    return rn
+
+
+def _check_scan(g, r, ref, reads):
+    gs_, gl_, st = g.scan(*reads_pool(reads))
+    rs_ = np.array([r.has_hit_in_set(x, 0) for x in reads], dtype=np.int8)
+    rl_ = np.array([ref.is_low_complexity(x) for x in reads], dtype=np.uint8)
+    assert (gl_ == rl_).all() and (gs_ == rs_).all(), ("scan", np.flatnonzero(gs_ != rs_)[:5], np.flatnonzero(gl_ != rl_)[:5])
+    assert st["with_hit"] == int((rs_ != 0).sum())
+    return int((rs_ != 0).sum())
+
+
+def check_refset_error_isolation(lib, ref, tmp_path, batch, seed=146):
+    """A read that fails on the device (more hits than the per-read scratch) fails its own call with T4_E_NOMEM, and only
+    that call: later get_overlaps, annotate and scan calls on the same gene set -- the annotate and scan launches reuse the
+    same worker shells, `batch` reads keep their count unchanged -- answer as the reference does.  A batch that contains
+    the failing read fails as a whole."""
+    fa = os.path.join(str(tmp_path), "genes_bad%d.fa" % seed)
+    recs = write_bad_gene_fasta(fa)
+    lib.check(lib.reset())
+    g = api.RefSet(fa, 9, lib, hit_len_required=31)
+    r = ref.RefGeneSet(fa, 9, hit_len_required=31)
+    good = annotate_reads(recs, batch, seed)
+    ann = [r.annotate_read(t) for t in good]
+    pool, off, lens = reads_pool(good)
+    with_bad = lambda j: reads_pool(good[:j] + [BAD_READ] + good[j + 1:])
+    nonempty = [t for t, a in zip(good, ann) if (a[0][:, 0] >= 0).any()][:6]
+    assert len(nonempty) >= 3
+    for t in nonempty[:2]:
+        _check_overlaps_read(g, r, t)
+    _expect_error(api.T4_E_NOMEM, g.get_overlaps, BAD_READ)
+    assert sum(_check_overlaps_read(g, r, t) for t in nonempty) > 0
+    _expect_error(api.T4_E_NOMEM, g.annotate, *with_bad(0))
+    compare_annotations(*g.annotate(pool, off, lens), good, ann, "after a failed annotate")
+    _expect_error(api.T4_E_NOMEM, g.annotate, *with_bad(batch // 2))
+    assert _check_scan(g, r, ref, good) > batch // 4
+    compare_annotations(*g.annotate(pool, off, lens), good, ann, "after a failed annotate and a scan")
+    _expect_error(api.T4_E_NOMEM, g.get_overlaps, BAD_READ)
+    _expect_error(api.T4_E_NOMEM, g.annotate, *with_bad(batch - 1))
+    for t in nonempty:
+        _check_overlaps_read(g, r, t)
+    compare_annotations(*g.annotate(pool, off, lens), good, ann, "at the end")
+    g.close()
+
+
+def check_refset_annotate_batches(lib, ref, tmp_path, n_workers, seed=144):
+    """t4_refset_annotate at batch sizes around the worker count (one read, fewer reads than workers, one short, exactly as
+    many, one more, three rounds and a few): every read against the reference; n = 0 returns 0; the largest batch twice on
+    the same set gives byte-identical output (results do not depend on which worker took which read)."""
+    fa = os.path.join(str(tmp_path), "genes_b%d.fa" % seed)
+    recs = write_gene_fasta(fa)
+    lib.check(lib.reset())
+    g = api.RefSet(fa, 9, lib, hit_len_required=31)
+    r = ref.RefGeneSet(fa, 9, hit_len_required=31)
+    sizes = sorted(set([1, 37, n_workers - 1, n_workers, n_workers + 1, 3 * n_workers + 5]) - {0})
+    reads = annotate_reads(recs, max(sizes) + 101, seed)
+    ann = [r.annotate_read(t) for t in reads]
+    z = np.zeros(16, dtype=np.uint8)
+    zo = np.zeros(1, dtype=np.uint64)
+    zl = np.zeros(1, dtype=np.int32)
+    out = np.zeros((1, 4, 8), dtype=np.int32)
+    sim = np.zeros((1, 4), dtype=np.float64)
+    assert lib.refset_annotate(g.h, z.ctypes.data, z.nbytes, zo.ctypes.data, zl.ctypes.data, 0, out.ctypes.data, sim.ctypes.data) == 0
+    for j, n in enumerate(sizes):
+        s0 = (j * 17) % (len(reads) - n + 1)
+        part = reads[s0:s0 + n]
+        go, gsim = g.annotate(*reads_pool(part))
+        compare_annotations(go, gsim, part, ann[s0:s0 + n], "n=%d" % n)
+    part = reads[: max(sizes)]
+    pool, off, lens = reads_pool(part)
+    a1, s1 = g.annotate(pool, off, lens)
+    a2, s2 = g.annotate(pool, off, lens)
+    assert a1.tobytes() == a2.tobytes() and s1.tobytes() == s2.tobytes()
+    n_set = compare_annotations(a1, s1, part, ann[: max(sizes)], "repeat")
+    assert n_set[0] > len(part) // 5, n_set
+    g.close()
+    return sizes
+
+
+def check_refset_interleaved(lib, ref, tmp_path, n, seed=145):
+    """scan -> annotate -> scan -> get_overlaps -> annotate on one gene set: the scan and annotate launches share the worker
+    shells (the annotate also writes their key buffers); every result must equal the reference's."""
+    fa = os.path.join(str(tmp_path), "genes_i%d.fa" % seed)
+    recs = write_gene_fasta(fa)
+    lib.check(lib.reset())
+    g = api.RefSet(fa, 9, lib, hit_len_required=31)
+    r = ref.RefGeneSet(fa, 9, hit_len_required=31)
+    ra = annotate_reads(recs, n, seed)
+    rb = annotate_reads(recs, n, seed + 1000)
+    assert _check_scan(g, r, ref, rb) > n // 4
+    compare_annotations(*g.annotate(*reads_pool(ra)), ra, [r.annotate_read(t) for t in ra], "first annotate")
+    assert _check_scan(g, r, ref, ra) > n // 4
+    assert sum(_check_overlaps_read(g, r, t) for t in rb[:200]) > 100
+    n_set = compare_annotations(*g.annotate(*reads_pool(rb)), rb, [r.annotate_read(t) for t in rb], "second annotate")
+    assert n_set[0] > n // 5, n_set
+    g.close()
+
+
+def example_reads():
+    """The reads of the shipped example (tests/golden/example_{1,2}.fq.gz), both mates, in file order."""
+    out = []
+    for m in (1, 2):
+        lines = gzip.open(os.path.join(GOLD, "example_%d.fq.gz" % m)).read().decode().split("\n")
+        out.extend(lines[1::4][: len(lines) // 4])
+    return out
+
+
+def check_refset_annotate_example(lib, ref, tmp_path):
+    """The rough annotation of the shipped example's 396 reads against the reference's own hg38 gene set
+    (tests/golden/hg38_bcrtcr.fa.gz): real reads and real IMGT genes, with C genes and their names."""
+    fa = os.path.join(str(tmp_path), "hg38_bcrtcr.fa")
+    with open(fa, "wb") as f:
+        f.write(gzip.open(os.path.join(GOLD, "hg38_bcrtcr.fa.gz")).read())
+    reads = example_reads()
+    assert len(reads) == 396
+    lib.check(lib.reset())
+    g = api.RefSet(fa, 9, lib, hit_len_required=17)
+    r = ref.RefGeneSet(fa, 9, hit_len_required=17)
+    assert g.names() == r.names()
+    n_set = compare_annotations(*g.annotate(*reads_pool(reads)), reads, [r.annotate_read(t) for t in reads], "example")
+    assert n_set[0] > 100 and n_set[2] > 50, n_set
+    for t in reads[::9]:
+        _check_overlaps_read(g, r, t)
+    g.close()
+    return n_set

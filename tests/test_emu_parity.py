@@ -139,3 +139,43 @@ def test_emu_sort_reads(emu_lib, ref):
 def test_emu_mate_overlap(emu_lib, ref):
     """SURVEY.md 8f-3, mate read-through / merge detection: AlignAlgo::IsMateOverlap per pair (emulation only)."""
     assert pc.check_mate_overlap(emu_lib, ref) > 600
+
+
+@pytest.mark.parametrize("seed,radius,hit_len,k", [(134, None, 31, 11), (135, 0, 17, 7)])
+def test_emu_refset_overlaps_other_k(emu_lib, ref, tmp_path, seed, radius, hit_len, k):
+    """GetOverlapsFromRead on gene sets indexed at k = 11 and at k = 7 with hitLenRequired 17 (the --trimLevel 2 re-index)."""
+    assert pc.check_refset_overlaps(emu_lib, ref, tmp_path, seed=seed, n=300, radius=radius, hit_len=hit_len, k=k) > 300
+
+
+def test_emu_refset_annotate_example(emu_lib, ref, tmp_path):
+    """AnnotateRead of the shipped example's reads on the reference's hg38 gene set."""
+    pc.check_refset_annotate_example(emu_lib, ref, tmp_path)
+
+
+def test_emu_refset_annotate_batches(emu_lib, ref, tmp_path):
+    """Batch sizes around the emulation's worker count (2), n = 0, a repeated batch byte for byte."""
+    pc.check_refset_annotate_batches(emu_lib, ref, tmp_path, n_workers=2)
+
+
+def test_emu_refset_interleaved(emu_lib, ref, tmp_path):
+    pc.check_refset_interleaved(emu_lib, ref, tmp_path, n=300)
+
+
+def test_emu_refset_error_isolation(emu_lib, ref, tmp_path):
+    """A read over the per-read hit limit fails its own call only; the gene set and its worker shells stay usable."""
+    pc.check_refset_error_isolation(emu_lib, ref, tmp_path, batch=12)
+
+
+def test_emu_sort_reads_edges(emu_lib, ref):
+    """Bytes >= 0x80, reads over 512 bp, avg one ulp apart and -0.0 / 0.0, groups of records equal in every field."""
+    assert pc.check_sort_reads_edges(emu_lib, ref, n_base=600) > 1000
+
+
+def test_emu_sort_reads_python_key(emu_lib):
+    """The sort against the plain Python restatement of the comparator, ragged size."""
+    assert pc.check_sort_reads_large(emu_lib, n=20011) == 20011
+
+
+def test_emu_mate_overlap_edges(emu_lib, ref):
+    """Zero-length mates, minOverlap >= flen and 0, the threshold steps at 50 / 100 bases, N's, lower case, tandem repeats."""
+    assert pc.check_mate_overlap_edges(emu_lib, ref, reps=3) > 200

@@ -9,9 +9,10 @@
 //                              AlignAlgo::GlobalAlignment, indels allowed, similarity >= refSeqSimilarity
 //                                                                                              SeqSet.hpp:1508-2124, AlignAlgo.hpp:218-420
 //
-// STATUS: verified against the reference through the test emulation only (tests/test_emu_parity.py); it was written
-// after the round's GPU budget had ended, runs in a kernel of its own (t4_annot_kernel) so that the GPU-validated kernels
-// keep their exact SASS, and has no GPU test yet.  Probe and key sort are the engine's collectives; everything after is
+// STATUS: verified on an H100 against the compiled reference through t4_refset_get_overlaps and t4_refset_annotate
+// (tests/test_gpu_preprocess.py: 528 workers on one read cursor, batch sizes around the worker count, the shipped example
+// on the reference's hg38 gene set, interleaved scan / annotate / get-overlaps calls), and through the test emulation.  It
+// runs in a kernel of its own (t4_annot_kernel).  Probe and key sort are the engine's collectives; everything after is
 // serial per read on thread 0 in plain C (shared with the emulation).
 #ifndef T4_ANNOT_H
 #define T4_ANNOT_H

@@ -73,8 +73,8 @@ __global__ void __launch_bounds__( T4_MAX_NT, T4_MIN_BLOCKS ) t4_aux_kernel( cha
 	c_run_aux_op( cx, ops + blockIdx.x ) ;
 }
 
-// GetOverlapsFromRead on a reference gene set (t4_annot.h): a kernel of its own, so that the kernels validated on the GPU
-// keep their exact SASS while this one is verified through the emulation only
+// GetOverlapsFromRead and AnnotateRead on a reference gene set (t4_annot.h): a kernel of its own, so that the other op
+// kernels keep their exact SASS
 __global__ void __launch_bounds__( T4_MAX_NT, T4_MIN_BLOCKS ) t4_annot_kernel( char *A, T4Op *ops )
 {
 	__shared__ T4Smem sm ;
@@ -82,7 +82,7 @@ __global__ void __launch_bounds__( T4_MAX_NT, T4_MIN_BLOCKS ) t4_annot_kernel( c
 	c_run_annot_op( cx, ops + blockIdx.x ) ;
 }
 
-// one merge pass of the read sort (t4_readsort.h); emulation-verified only, like t4_annot_kernel
+// one merge pass of the read sort (t4_readsort.h)
 __global__ void t4_readsort_kernel( T4SortParams P )
 {
 	for ( i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x ; i < P.n ; i += (i64)gridDim.x * blockDim.x )
@@ -2012,7 +2012,8 @@ struct t4_refset
 {
 	t4_seqset *set ;                   // the sequences as contigs of one stream, indexed at k
 	std::vector<std::string> names ;   // after the de-duplication ("a|b" for identical sequences, SeqSet.hpp:2751-2760)
-	std::vector<t4_seqset *> workers ; // scratch-only streams of the scan launch (created on first use)
+	std::vector<t4_seqset *> workers ; // scratch-only streams of the scan and annotate launches (created on first use)
+	u64 workerPitch ;                  // arena distance between consecutive worker shells (one seqsets_create_impl call)
 	char *dbuf ;                       // device: parameter block + op records of the scan launch
 	size_t dbufCap ;
 	int k ;
@@ -2152,7 +2153,7 @@ t4_refset *T4_API( refset_create_from_fa )( const char *fasta_path, int kmer_len
 		return 0 ;
 	}
 	t4_refset *r = new t4_refset ;
-	r->set = 0 ; r->k = kmer_length ; r->gen = g_gen ; r->dbuf = 0 ; r->dbufCap = 0 ;
+	r->set = 0 ; r->k = kmer_length ; r->gen = g_gen ; r->workerPitch = 0 ; r->dbuf = 0 ; r->dbufCap = 0 ;
 	if ( seqsets_create_impl( 1, kmer_length, 31, 0, &r->set ) )
 	{
 		delete r ;
@@ -2247,7 +2248,26 @@ static int refset_workers( t4_refset *r, int n )
 	int rc = seqsets_create_impl( n, r->k, 31, 0, r->workers.data() ) ;
 	if ( rc )
 		r->workers.clear() ;
+	else
+		r->workerPitch = n > 1 ? r->workers[1]->off - r->workers[0]->off : sizeof( T4Stream ) ;
 	return rc ;
+}
+
+// Clears the device error word (error, errorAux) of the first n worker shells, ordered on `stream` before the launch that
+// uses them.  A read that fails (e.g. more hits than the per-read scratch holds) fails its own call; the shells are reused
+// by every later scan and annotate of the refset, which must not inherit that error.
+static int refset_clear_worker_errors( t4_refset *r, int n, void *stream )
+{
+	char *first = E.A + r->workers[0]->off + offsetof( T4Stream, error ) ;
+	static_assert( offsetof( T4Stream, errorAux ) == offsetof( T4Stream, error ) + sizeof( int ), "error word layout" ) ;
+#if T4_CUDA
+	CK( cudaMemset2DAsync( first, r->workerPitch, 0, 2 * sizeof( int ), n, (cudaStream_t)stream ) ) ;
+#else
+	(void)stream ;
+	for ( int w = 0 ; w < n ; ++w )
+		memset( first + (size_t)w * r->workerPitch, 0, 2 * sizeof( int ) ) ;
+#endif
+	return 0 ;
 }
 
 // Host read records: read i is pool[seq_off[i] .. + len[i]).  fn names the entry point in the message.
@@ -2315,7 +2335,7 @@ int T4_API( refset_scan_device )( t4_refset *r, const void *pool, const void *se
 		x.out = (u64)(uintptr_t)r->dbuf ;
 	}
 	if ( ( rc = h2d_async( r->dbuf, &P, sizeof( P ), cuda_stream ) ) || ( rc = h2d_async( r->dbuf + 256, ops.data(), (size_t)n_workers * sizeof( T4Op ), cuda_stream ) )
-		|| ( rc = dzero( ctrl, 32, cuda_stream ) ) )
+		|| ( rc = dzero( ctrl, 32, cuda_stream ) ) || ( rc = refset_clear_worker_errors( r, n_workers, cuda_stream ) ) )
 		return rc ;
 	return launch_ops( T4K_AUX, (T4Op *)( r->dbuf + 256 ), n_workers, cuda_stream ) ;
 }
@@ -2348,9 +2368,10 @@ int T4_API( refset_scan )( t4_refset *r, const char *read_pool, size_t pool_byte
 	if ( !rc ) rc = h2d( dPool, read_pool, pool_bytes ) ;
 	if ( !rc ) rc = h2d( dOff, seq_off, (size_t)n * 8 ) ;
 	if ( !rc ) rc = h2d( dLen, len, (size_t)n * 4 ) ;
-	if ( !rc ) rc = T4_API( refset_scan_device )( r, dPool, dOff, dLen, n, dStr, dLow, dCtrl, 0, 0 ) ;
+	const int nw = resident_workers() ;
+	if ( !rc ) rc = T4_API( refset_scan_device )( r, dPool, dOff, dLen, n, dStr, dLow, dCtrl, nw, 0 ) ;
 	if ( !rc ) rc = dsync() ;
-	if ( !rc ) rc = T4_API( streams_error )( r->workers.data(), (int)r->workers.size() ) ;
+	if ( !rc ) rc = T4_API( streams_error )( r->workers.data(), nw ) ;
 	if ( !rc && strand_out ) rc = d2h( strand_out, dStr, (size_t)n ) ;
 	if ( !rc && low_complexity_out ) rc = d2h( low_complexity_out, dLow, (size_t)n ) ;
 	if ( !rc && stats )
@@ -2365,7 +2386,7 @@ int T4_API( refset_scan )( t4_refset *r, const char *read_pool, size_t pool_byte
 // SeqSet::GetOverlapsFromRead( read, 0, -1, 0, false, overlaps ) on the reference gene set (the call AnnotateRead makes per
 // read, SeqSet.hpp:6050): overlaps as int32[8] = {seqIdx, readStart, readEnd, seqStart, seqEnd, strand, matchCnt, indelCnt}
 // plus similarity[i], in the reference's order.  Returns the overlap count, -1 for a read shorter than k.
-// NOTE: verified through the test emulation only (see t4_annot.h).
+// Verified on the GPU against the reference (see t4_annot.h).
 int T4_API( refset_get_overlaps )( t4_refset *r, const char *read, int32_t *overlaps, double *similarity, int cap )
 {
 	int rc = refset_check( r ) ;
@@ -2378,6 +2399,11 @@ int T4_API( refset_get_overlaps )( t4_refset *r, const char *read, int32_t *over
 	T4Stream st ;
 	rc = get_stream( r->set, &st ) ;
 	if ( rc ) return rc ;
+	if ( st.error ) // raised by something other than an earlier get_overlaps (those clear it below): still reported
+	{
+		set_err( "t4_refset_get_overlaps: the gene set carries device error " + std::to_string( st.error ) + " aux " + std::to_string( st.errorAux ) ) ;
+		return st.error ;
+	}
 	const int hMax = 1 << 16 ;
 	const size_t sb = t4_annot_scratch_bytes( hMax, st.nomatchGapLimit, T4_DEV_MAX_READ ) ;
 	DevBuf m ;
@@ -2417,14 +2443,23 @@ int T4_API( refset_get_overlaps )( t4_refset *r, const char *read, int32_t *over
 	}
 	if ( rc ) return rc ;
 	if ( n < T4_E_BASE )
-		set_err( "t4_refset_get_overlaps: device error " + std::to_string( n ) ) ;
+	{
+		// the op runs on the set's own stream, so the error this read raised sits in the set's error word: report it, then
+		// clear the word so that the next read is answered on its own
+		rc = get_stream( r->set, &st ) ;
+		if ( rc ) return rc ;
+		set_err( "t4_refset_get_overlaps: device error " + std::to_string( n ) + " aux " + std::to_string( st.errorAux ) ) ;
+		const int clear[2] = { 0, 0 } ;
+		rc = put_field( r->set, offsetof( T4Stream, error ), clear, sizeof( clear ) ) ;
+		if ( rc ) return rc ;
+	}
 	return n ;
 }
 
 // SeqSet::AnnotateRead( read, 0, geneOverlap, NULL, NULL ) for every read (the rough annotation of the stage-1 driver,
 // main.cpp:1084-1120; SeqSet.hpp:6016-6340): gene_overlaps[i][t][8] for t = V, D, J, C = {seqIdx (-1: none), readStart,
 // readEnd, seqStart, seqEnd, strand, matchCnt, indelCnt}, similarity[i][t].  Host buffers.
-// NOTE: verified through the test emulation only (see t4_annot.h).
+// Verified on the GPU against the reference (see t4_annot.h).
 int T4_API( refset_annotate )( t4_refset *r, const char *read_pool, size_t pool_bytes, const uint64_t *seq_off, const int32_t *len, int64_t n,
 	int32_t *gene_overlaps, double *similarity )
 {
@@ -2482,6 +2517,7 @@ int T4_API( refset_annotate )( t4_refset *r, const char *read_pool, size_t pool_
 	if ( !rc ) rc = h2d( dOff, seq_off, (size_t)n * 8 ) ;
 	if ( !rc ) rc = h2d( dLen, len, (size_t)n * 4 ) ;
 	if ( !rc ) rc = dzero( dCtrl, 64 ) ;
+	if ( !rc ) rc = refset_clear_worker_errors( r, nw, 0 ) ;
 	if ( !rc ) rc = launch_ops( T4K_ANNOT, dOps, nw, 0 ) ;
 	if ( !rc ) rc = dsync() ;
 	if ( !rc ) rc = T4_API( streams_error )( r->workers.data(), nw ) ;
@@ -2492,7 +2528,7 @@ int T4_API( refset_annotate )( t4_refset *r, const char *read_pool, size_t pool_
 
 // `std::sort( sortedReads.begin(), sortedReads.end() )` of the stage-1 driver (main.cpp:1078; _sortRead::operator<, :103-125):
 // order[j] = index of the record that comes j-th.  Host buffers; record i: read_pool[seq_off[i] .. + len[i]), its id
-// id_pool[id_off[i] .. id_off[i + 1]), its count statistics.  NOTE: verified through the test emulation only (t4_readsort.h).
+// id_pool[id_off[i] .. id_off[i + 1]), its count statistics.  Verified on the GPU (t4_readsort.h).
 int T4_API( sort_reads )( const char *read_pool, size_t pool_bytes, const uint64_t *seq_off, const int32_t *len, const char *id_pool,
 	size_t id_pool_bytes, const uint64_t *id_off, const int32_t *min_cnt, const int32_t *median_cnt, const float *avg_cnt, int64_t n,
 	int64_t *order )
@@ -2548,7 +2584,7 @@ int T4_API( sort_reads )( const char *read_pool, size_t pool_bytes, const uint64
 
 // AlignAlgo::IsMateOverlap for n (first, second) read pairs of one pool (ProcessRead, main.cpp:264, 291): overlap_size[i] =
 // the return value (-1: no unambiguous overlap), offset[i] / best_match_cnt[i] the two reference outputs.  Host buffers.
-// NOTE: verified through the test emulation only (t4_readsort.h).
+// Verified on the GPU against the reference (t4_readsort.h).
 int T4_API( mate_overlap_batch )( const char *read_pool, size_t pool_bytes, const uint64_t *f_off, const int32_t *f_len, const uint64_t *s_off,
 	const int32_t *s_len, const int32_t *min_overlap, const uint8_t *check_tandem, int64_t n, int32_t *overlap_size, int32_t *offset,
 	int32_t *best_match_cnt )

@@ -7,8 +7,9 @@
 // elements of its pair of runs by ONE binary search in the partner run (lower bound for the left run's elements, upper
 // bound for the right run's: stable) -- n independent searches per pass, log2 n passes, no shared state.
 //
-// STATUS: verified against the reference comparator through the test emulation only (written after the round's GPU budget
-// had ended); a kernel of its own (t4_readsort_kernel), no GPU test yet.
+// STATUS: verified on an H100 (tests/test_gpu_preprocess.py) against the reference's std::sort and, at 2^20 + 3 records
+// (more than one grid of the grid-stride loop), against a Python restatement of the comparator; a kernel of its own
+// (t4_readsort_kernel).
 #ifndef T4_READSORT_H
 #define T4_READSORT_H
 
@@ -110,7 +111,7 @@ T4_HD inline void t4_sort_merge_one( const T4SortParams &P, i64 i )
 // AlignAlgo::IsMateOverlap( fr, flen, sr, slen, minOverlap, offset, bestMatchCnt, checkTandem ) (AlignAlgo.hpp:1027-1096) as
 // ProcessRead calls it for every read pair (main.cpp:264, 291): does a suffix of `fr` match a prefix of `sr` at exactly one
 // offset (similarity threshold 0.85 ... 0.95 by length), and is the match not a tandem repeat?  One thread per pair.
-// Same emulation-only status as the sort above.
+// Verified on an H100 pair by pair against the reference: 300 000 pairs (more than one grid) and the function's edges.
 struct T4MateParams
 {
 	u64 pool ;             // ASCII reads
