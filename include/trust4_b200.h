@@ -140,7 +140,11 @@ int t4_dp_pos_weight_batch(int n, const int32_t *t_weights, const int64_t *t_off
 /* The same alignment through the two routines the stream kernel actually runs for its equal-length problems
  * (overhangs of ExtendOverlap, SeqSet.hpp:1165; same-diagonal gaps of GetOverlapsFromRead, SeqSet.hpp:1832-2006):
  * variant 0 = per-thread register banded DP, variant 1 = half-warp anti-diagonal DP (no <=2-mismatch fast path:
- * its caller settles those from popcounts).  Problem i spans columns/bases off[i]..off[i+1) of both inputs. */
+ * its caller settles those from popcounts), variant 2 = ExtendOverlap's overhang pass: problems 2k and 2k+1 run on the
+ * two halves of one warp as a left overhang (statistics taken from its end) and a right one, and instead of the edit
+ * string align_out receives at align_off[i] (a multiple of 4, 16 bytes) four int32: the matches, mismatches and indels
+ * of the alignment and its good-prefix length (SeqSet.hpp:1176-1224); score_out is not written.  Variants 1 and 2 exist
+ * only in the CUDA build.  Problem i spans columns/bases off[i]..off[i+1) of both inputs. */
 int t4_dp_hot_path_batch(int n, int variant, const int32_t *t_weights, const int64_t *off, const char *p,
                          int8_t *align_out, const int64_t *align_off, int32_t *score_out);
 
@@ -267,7 +271,9 @@ int64_t t4_seqset_index_checksum(t4_seqset *s, uint64_t *checksum);
  * [4] hits emitted (sum c_j'), [5] packed read bytes ceil(L/4), [6] overlaps scored, [7] gap DPs,
  * [8..15] clock cycles per phase: other, probe, hit sort, chains, scoring, ExtendOverlap, decide+commit,
  * InputNovelRead/RepeatAddRead/consensus; [16] overlaps extended; [17..19] cycles inside ExtendOverlap (bit masks,
- * classification, DPs), [20] reads taking the lazy ExtendOverlap path; [21..23] reserved. */
+ * classification, DPs), [20] reads taking the lazy ExtendOverlap path; [21] ExtendOverlaps the decision loop still runs
+ * on demand on its single thread (s_make_exact: overlaps it consults without a result), [22] the clock cycles they take;
+ * [23] reserved. */
 #define T4_N_COUNTERS 24
 int t4_last_counters(uint64_t *counters /* T4_N_COUNTERS */);
 

@@ -345,7 +345,8 @@ def dp_pos_weight_batch(problems, lib: Lib | None = None):
 
 
 def dp_hot_path_batch(problems, variant, lib: Lib | None = None):
-    """Equal-length problems through the hot-path DP routines (t4_dp_hot_path_batch).  Returns [(score, [edit ops])]."""
+    """Equal-length problems through the hot-path DP routines (t4_dp_hot_path_batch).  Returns [(score, [edit ops])];
+    variant 2 (problems 2k, 2k+1 = a left and a right overhang side on one warp) returns [(matches, mismatches, indels, good)]."""
     lib = lib or default_lib()
     n = len(problems)
     off = np.zeros(n + 1, dtype=np.int64)
@@ -353,7 +354,7 @@ def dp_hot_path_batch(problems, variant, lib: Lib | None = None):
     for i, (tw, p) in enumerate(problems):
         assert len(tw) == len(p)
         off[i + 1] = off[i] + len(p)
-        a_off[i + 1] = a_off[i] + 2 * len(p) + 2
+        a_off[i + 1] = a_off[i] + ((max(2 * len(p) + 2, 16) + 3) & ~3)
     tw_all = np.zeros((max(1, off[n]), 4), dtype=np.int32)
     for i, (tw, p) in enumerate(problems):
         tw_all[off[i]:off[i + 1]] = tw
@@ -362,6 +363,8 @@ def dp_hot_path_batch(problems, variant, lib: Lib | None = None):
     score = np.zeros(n, dtype=np.int32)
     lib.check(lib.dp_hot_path_batch(n, variant, tw_all.ctypes.data, off.ctypes.data, p_all.ctypes.data,
                                     align.ctypes.data, a_off.ctypes.data, score.ctypes.data))
+    if variant == 2:
+        return [tuple(int(v) for v in align[a_off[i]:a_off[i] + 16].view(np.int32)) for i in range(n)]
     out = []
     for i in range(n):
         e = []

@@ -144,15 +144,54 @@ __global__ void t4_pack_kernel( char *A, const u64 *streamOff, const u64 *outOff
 // Test entry for the two DP routines the stream kernel really runs (equal lengths: overhangs and same-diagonal gaps):
 // variant 0 = t4_dp_equal (register-resident banded DP, one thread per problem, ExtendOverlap),
 // variant 1 = w_stage_side + w_dp_equal_half (half-warp anti-diagonal DP over staged IsBaseEqual nibbles, gap scoring;
-//             it has no fast path: the caller only runs it when the diagonal has > 2 mismatches).
-// One warp per problem.  scratch: per problem 13 * actStride u32 traceback words + an edit-string buffer (large n).
+//             it has no fast path: the caller only runs it when the diagonal has > 2 mismatches),
+// variant 2 = w_side_pair (ExtendOverlap's overhang pass: problems 2k and 2k+1 on the two halves of warp k, as a left
+//             side, scanned from its end, and a right side); writes each problem's T4SideStats, not its edit string.
+// One warp per problem (variant 2: per pair).  scratch: per problem 13 * actStride u32 traceback words + an edit-string
+// buffer (large n).
 __global__ void t4_dp_hot_kernel( int n, int variant, const int *tw, const i64 *off, const char *p, signed char *align, const i64 *alignOff,
 	int *score, u32 *scratch, const i64 *scratchOff )
 {
-	__shared__ u32 nib[64] ;
-	__shared__ u32 bits[16] ;
+	__shared__ u32 nib[2][64] ;
+	__shared__ u32 bits[2][16] ;
 	__shared__ u32 act[2][13 * T4_WACT_WORDS] ;
 	__shared__ signed char wal[2][2 * 16 * T4_WACT_WORDS + 8] ;
+	if ( variant == 2 )
+	{
+		T4Ctx cx ;
+		cx.tid = threadIdx.x ;
+		cx.nt = 32 ;
+		T4DpSide s[2] ;
+		for ( int h = 0 ; h < 2 ; ++h )
+		{
+			const int k = 2 * blockIdx.x + h ;
+			T4DpSide &d = s[h] ;
+			d.n = ( k < n ) ? (int)( off[k + 1] - off[k] ) : 0 ;
+			d.tw = tw + 4 * off[k < n ? k : 0] ;
+			d.p = p + off[k < n ? k : 0] ;
+			d.fromEnd = ( h == 0 ) ;
+			const bool small = d.n < 16 * T4_WACT_WORDS ;
+			d.actStride = small ? T4_WACT_WORDS : ( d.n / 16 + 2 ) ;
+			d.act = small ? act[h] : scratch + scratchOff[k] ;
+			d.alCap = small ? (int)sizeof( wal[0] ) : 2 * d.n + 8 ;
+			d.al = small ? wal[h] : (signed char *)( scratch + scratchOff[k] + 13 * d.actStride ) ;
+		}
+		T4SideStats r[2] ;
+		w_side_pair( cx, s[0], s[1], nib, bits, r[0], r[1] ) ;
+		for ( int h = 0 ; h < 2 ; ++h )
+		{
+			const int k = 2 * blockIdx.x + h ;
+			if ( threadIdx.x == 0 && k < n )
+			{
+				int *o = (int *)( align + alignOff[k] ) ;
+				o[0] = r[h].m ;
+				o[1] = r[h].x ;
+				o[2] = r[h].ind ;
+				o[3] = r[h].good ;
+			}
+		}
+		return ;
+	}
 	int i = blockIdx.x ;
 	if ( i >= n )
 		return ;
@@ -170,7 +209,7 @@ __global__ void t4_dp_hot_kernel( int n, int variant, const int *tw, const i64 *
 	T4Ctx cx ;
 	cx.tid = lane ;
 	cx.nt = 32 ;
-	int matches = w_stage_side( t, pp, len, nib, bits, lane ) ;
+	int matches = w_stage_side( t, pp, len, nib[0], bits[0], lane ) ;
 	(void)matches ;
 	const bool small = len < 16 * T4_WACT_WORDS ;
 	const int actStride = small ? T4_WACT_WORDS : ( len / 16 + 2 ) ;
@@ -178,7 +217,7 @@ __global__ void t4_dp_hot_kernel( int n, int variant, const int *tw, const i64 *
 	const int acap = small ? (int)sizeof( wal[0] ) : 2 * len + 8 ;
 	signed char *abuf = small ? wal[lane < 16 ? 0 : 1] : (signed char *)( scratch + scratchOff[i] + 26 * actStride ) + ( lane < 16 ? 0 : acap ) ;
 	int alen = 0 ;
-	int sc = w_dp_equal_half( cx, nib, pp, lane < 16 ? len : 0, abuf, acap, &alen, actBase, actStride ) ;
+	int sc = w_dp_equal_half( cx, nib[0], pp, lane < 16 ? len : 0, abuf, acap, &alen, actBase, actStride ) ;
 	alen = __shfl_sync( 0xffffffffu, alen, 0 ) ;
 	sc = __shfl_sync( 0xffffffffu, sc, 0 ) ;
 	signed char *buf0 = small ? wal[0] : (signed char *)( scratch + scratchOff[i] + 26 * actStride ) ;
@@ -1340,7 +1379,7 @@ int T4_API( dp_pos_weight_batch )( int n, const int32_t *t_weights, const int64_
 }
 
 // The hot-path DP routines on n equal-length problems (problem i: columns / bases off[i]..off[i+1)).
-// variant 0: t4_dp_equal; variant 1: w_dp_equal_half (product build only).
+// variant 0: t4_dp_equal; variant 1: w_dp_equal_half; variant 2: w_side_pair (1 and 2: product build only).
 int T4_API( dp_hot_path_batch )( int n, int variant, const int32_t *t_weights, const int64_t *off, const char *p, int8_t *align_out,
 	const int64_t *align_off, int32_t *score_out )
 {
@@ -1348,12 +1387,12 @@ int T4_API( dp_hot_path_batch )( int n, int variant, const int32_t *t_weights, c
 	if ( r ) return r ;
 	if ( n <= 0 )
 		return 0 ;
-	if ( variant != 0 && variant != 1 )
+	if ( variant < 0 || variant > 2 )
 		return T4_E_INVAL ;
 #if !T4_CUDA
-	if ( variant == 1 )
+	if ( variant != 0 )
 	{
-		set_err( "w_dp_equal_half exists only in the CUDA build" ) ;
+		set_err( "the warp DP routines exist only in the CUDA build" ) ;
 		return T4_E_UNSUPPORTED ;
 	}
 #endif
@@ -1365,7 +1404,9 @@ int T4_API( dp_hot_path_batch )( int n, int variant, const int32_t *t_weights, c
 		so[i] = tot ;
 		i64 stride = len / 16 + 2 ;
 		tot += 26 * stride + ( 2 * ( 2 * len + 8 ) + 3 ) / 4 + len + 8 ; // u32 words: traceback of both halves, edit strings, act32 of variant 0
-		i64 e = align_off[i] + 2 * len + 2 ;
+		if ( variant == 2 && ( align_off[i] & 3 ) )
+			return T4_E_INVAL ;
+		i64 e = align_off[i] + ( ( variant == 2 && 2 * len + 2 < 16 ) ? 16 : 2 * len + 2 ) ;
 		if ( e > alignTot )
 			alignTot = e ;
 	}
@@ -1383,7 +1424,7 @@ int T4_API( dp_hot_path_batch )( int n, int variant, const int32_t *t_weights, c
 		|| ( r = h2d( dAo, align_off, szO ) ) || ( r = h2d( dSo, so.data(), szO ) ) )
 		return r ;
 #if T4_CUDA
-	t4_dp_hot_kernel<<<n, 32>>>( n, variant, dT, dOff, dP, dA, dAo, dS, dScr, dSo ) ;
+	t4_dp_hot_kernel<<<variant == 2 ? ( n + 1 ) / 2 : n, 32>>>( n, variant, dT, dOff, dP, dA, dAo, dS, dScr, dSo ) ;
 	CK( cudaGetLastError() ) ;
 	CK( cudaDeviceSynchronize() ) ;
 #else

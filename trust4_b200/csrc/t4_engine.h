@@ -2532,6 +2532,44 @@ T4_D inline T4SideStats w_side_stats( const T4AlignView &v, bool fromEnd, int la
 	return r ;
 }
 
+// One overhang side of w_side_pair: n columns tw[0..n) against p[0..n) (n == 0: no side); fromEnd for a left
+// overhang.  act / actStride: the traceback words of its half-warp DP; al / alCap: its edit-string buffer.
+struct T4DpSide
+{
+	const int *tw ;
+	const char *p ;
+	int n ;
+	bool fromEnd ;
+	u32 *act ;
+	int actStride ;
+	signed char *al ;
+	int alCap ;
+} ;
+
+// Two overhang alignments on one warp: both sides are staged, side h runs w_dp_equal_half on half-warp h (both halves
+// at once), then the whole warp takes each side's statistics from its edit string.  Results identical in every lane.
+T4_D inline void w_side_pair( T4Ctx &cx, const T4DpSide &s0, const T4DpSide &s1, u32 ( *nib )[64], u32 ( *bits )[16],
+	T4SideStats &r0, T4SideStats &r1 )
+{
+	const int lane = cx.tid & 31 ;
+	w_stage_side( s0.tw, s0.p, s0.n, nib[0], bits[0], lane ) ;
+	w_stage_side( s1.tw, s1.p, s1.n, nib[1], bits[1], lane ) ;
+	const bool hi = lane >= 16 ;
+	int alen = 0 ;
+	w_dp_equal_half( cx, nib[hi ? 1 : 0], hi ? s1.p : s0.p, hi ? s1.n : s0.n, hi ? s1.al : s0.al, hi ? s1.alCap : s0.alCap, &alen,
+		hi ? s1.act : s0.act, hi ? s1.actStride : s0.actStride ) ;
+	const int a0 = __shfl_sync( T4_FULL, alen, 0 ), a1 = __shfl_sync( T4_FULL, alen, 16 ) ;
+	T4AlignView v ;
+	v.bits = 0 ;
+	v.dp = 1 ;
+	v.a = s0.al + s0.alCap - 1 - a0 ;
+	v.n = a0 ;
+	r0 = w_side_stats( v, s0.fromEnd, lane ) ;
+	v.a = s1.al + s1.alCap - 1 - a1 ;
+	v.n = a1 ;
+	r1 = w_side_stats( v, s1.fromEnd, lane ) ;
+}
+
 T4_D inline signed char *t4_align_of_thread( T4Ctx &cx, int tid )
 {
 	return (signed char *)( cx.P<char>( cx.st->dpOff ) + (size_t)tid * cx.st->dpStride + 2 * T4_DP_W * 4 + 8
@@ -3226,6 +3264,9 @@ T4_D inline int c_dup_run_len( T4Ctx &cx, const t4_read_desc *descs, int i, int 
 // exact ExtendOverlap of overlap i on demand (thread 0 of the decision loop)
 T4_D inline void s_make_exact( T4Ctx &cx, const char *r, int len, double factor, const T4Ovl *overlaps, T4Ovl *pre, int i )
 {
+#if T4_CUDA
+	long long t0 = clock64() ;
+#endif
 	T4DpScratch ds = t4_dp_scratch( cx ) ;
 	const u32 *bits = cx.P<u32>( cx.st->bitsOff ) ;
 	T4Ovl e ;
@@ -3233,6 +3274,83 @@ T4_D inline void s_make_exact( T4Ctx &cx, const char *r, int len, double factor,
 	e.infoFromHits = ok ;
 	e.hcCnt = 2 ;
 	pre[i] = e ;
+	t4_count( cx, 21, 1 ) ;
+#if T4_CUDA
+	t4_count( cx, 22, (u64)( clock64() - t0 ) ) ;
+#endif
+}
+
+// Overhang side x = 2 i + right of overlap o = overlaps[i]: its posWeight columns *tw and read bases *p.  Returns its length.
+T4_D inline int t4_side_span( T4Ctx &cx, const T4Ovl &o, int right, const char *r, int len, const int **tw, const char **p )
+{
+	T4Contig *seq = t4_seq( cx, o.seqIdx ) ;
+	const int *pw = t4_pw( cx, seq ) ;
+	if ( !right )
+	{
+		int L = t4_min( o.readStart, o.seqStart ) ;
+		*tw = pw + 4 * ( o.seqStart - L ) ;
+		*p = r + o.readStart - L ;
+		return L ;
+	}
+	*tw = pw + 4 * ( o.seqEnd + 1 ) ;
+	*p = r + o.readEnd + 1 ;
+	return t4_min( len - 1 - o.readEnd, seq->len - 1 - o.seqEnd ) ;
+}
+
+// ExtendOverlap's overhang alignments of the sides pend[0 .. cnt) (each needs the banded DP): their statistics into
+// sstats[side].  Collective.  On the device each warp takes two sides at a time, one per half-warp (w_side_pair);
+// a side of 16 * T4_WACT_WORDS columns or more keeps its traceback and edit string in the arena scratch of its
+// half-warp's first thread instead of shared memory.  The emulation aligns them one at a time.
+T4_D inline void c_overhang_dps( T4Ctx &cx, const T4Ovl *overlaps, const char *r, int len, const u32 *bits, const int *pend, int cnt,
+	T4SideStats *sstats )
+{
+#if T4_CUDA
+	T4Smem *sm = cx.sm ;
+	const int warp = cx.tid >> 5, nwarps = cx.nt >> 5, lane = cx.tid & 31 ;
+	(void)bits ;
+	for ( int q = 2 * warp ; q < cnt ; q += 2 * nwarps )
+	{
+		T4DpSide s[2] ;
+#pragma unroll
+		for ( int h = 0 ; h < 2 ; ++h )
+		{
+			T4DpSide &d = s[h] ;
+			const int x = ( q + h < cnt ) ? pend[q + h] : -1 ;
+			d.tw = 0 ;
+			d.p = 0 ;
+			d.n = ( x >= 0 ) ? t4_side_span( cx, overlaps[x >> 1], x & 1, r, len, &d.tw, &d.p ) : 0 ;
+			d.fromEnd = !( x & 1 ) ;
+			const bool small = d.n < 16 * T4_WACT_WORDS ;
+			d.act = small ? sm->wact[warp][h] : (u32 *)t4_dp_scratch_of( cx, warp * 32 + 16 * h ).act ;
+			d.actStride = small ? T4_WACT_WORDS : (int)( T4_DP_STRIDE / 4 ) ;
+			d.al = small ? sm->wal[warp][h] : t4_align_of_thread( cx, warp * 32 + 16 * h ) ;
+			d.alCap = small ? (int)sizeof( sm->wal[0][0] ) : 2 * T4_DEV_MAX_READ + 8 ;
+		}
+		T4SideStats r0, r1 ;
+		w_side_pair( cx, s[0], s[1], sm->wnib[warp], sm->wbits[warp], r0, r1 ) ;
+		if ( lane == 0 )
+		{
+			sstats[pend[q]] = r0 ;
+			if ( q + 1 < cnt )
+				sstats[pend[q + 1]] = r1 ;
+			t4_count( cx, 1, ( q + 1 < cnt ) ? 2 : 1 ) ;
+		}
+	}
+#else
+	T4DpScratch ds = t4_dp_scratch( cx ) ;
+	T4_PAR_FOR( q, cnt )
+	{
+		const int x = pend[q] ;
+		const int *tw ;
+		const char *p ;
+		const int n = t4_side_span( cx, overlaps[x >> 1], x & 1, r, len, &tw, &p ) ;
+		T4AlignView av = t4_overhang_align( tw, p, n, bits + 32 * ( x >> 1 ) + 16 * ( x & 1 ), ds ) ;
+		if ( av.dp )
+			t4_count( cx, 1, 1 ) ;
+		sstats[x] = t4_side_stats( av, !( x & 1 ) ) ;
+	}
+#endif
+	T4_SYNC() ;
 }
 
 // IsBaseEqual( posWeight column, read base ) of every overhang column of every overlap (ExtendOverlap, SeqSet.hpp:1165-1175) as bit
@@ -3399,8 +3517,8 @@ T4_D T4_BIG int c_add_read( T4Ctx &cx, int len, const char *geneName, int &stran
 #endif
 		// Lazy ExtendOverlap.  One thread per (overlap, side) settles the sides that need no DP (<= 1 column, or <= 2
 		// mismatches on the diagonal, AlignAlgo.hpp:59-103) from the bit masks.  An overlap whose sides are all settled gets
-		// its exact result now (state 2).  Otherwise the DP is deferred: the decision loop below asks for the exact result
-		// only when it really consults it (s_make_exact); and when the return value alone matters (the bridging loop,
+		// its exact result now (state 2).  Otherwise its DP sides are deferred to the pass below (c_overhang_dps), which
+		// may leave an overlap to the decision loop to make exact on demand (s_make_exact); when the return value alone matters (the bridging loop,
 		// SeqSet.hpp:3736-3750) an overlap is skipped without any DP if ExtendOverlap provably returns 0 (state 1): with the
 		// total diagonal mismatch count M over the mismatch budget and density, either every deferred side aligns without
 		// indel (then its counts ARE the diagonal counts and the budget test fails) or some side has an indel (ret = 0).
@@ -3468,53 +3586,52 @@ T4_D T4_BIG int c_add_read( T4Ctx &cx, int len, const char *geneName, int &stran
 			pre[i] = e ;
 		}
 		T4_SYNC() ;
-		// Easy read: the best overlap is settled, extends, clears the threshold and covers the whole read.  The
-		// decision loop then consults the other overlaps (almost) only through the bridging loop, where state 1 suffices,
-		// and stragglers are made exact on demand.  Any other read: finish every deferred overlap now, one thread per
-		// (overlap, side) -- the decision loop may need many exact results and they must not serialise on thread 0.
+		// Every deferred side the decision loop may consult is aligned now, in one parallel pass, except the sides of a
+		// provably-0 overlap of an easy read (the best overlap is settled, extends, clears the threshold and covers the
+		// whole read).  The decision loop then consults the other overlaps (almost) only through the bridging loop,
+		// where state 1 suffices; the rare overlap it consults without a result is made exact on demand (s_make_exact).
 #if T4_CUDA
 		long long xt2 = clock64() ;
 #endif
 		bool easy = ( pre[0].hcCnt == 2 && pre[0].infoFromHits == 1 && pre[0].similarity >= similarityThreshold
 			&& pre[0].readStart == 0 && pre[0].readEnd == len - 1 ) ;
-		T4_SYNC() ;
-		if ( !easy )
+		int *pend = (int *)( sstats + 2 * overlapCnt ) ; // the sides to align, in side order (failOff holds a T4Ovl per overlap)
+#if T4_CUDA
+		if ( cx.tid < 32 )
 		{
-			T4DpScratch ds = t4_dp_scratch( cx ) ;
-			T4_PAR_FOR( x, 2 * overlapCnt )
+			int cnt = 0 ;
+			for ( int base = 0 ; base < 2 * overlapCnt ; base += 32 )
 			{
-				int i = x >> 1, right = x & 1 ;
-				if ( sstats[x].ind != -1 )
-					continue ;
-				const T4Ovl &o = overlaps[i] ;
-				T4Contig *seq = t4_seq( cx, o.seqIdx ) ;
-				int *pw = t4_pw( cx, seq ) ;
-				T4AlignView av ;
-				if ( !right )
-				{
-					int L = t4_min( o.readStart, o.seqStart ) ;
-					av = t4_overhang_align( pw + 4 * ( o.seqStart - L ), r + o.readStart - L, L, bits + 32 * i, ds ) ;
-				}
-				else
-				{
-					int R = t4_min( len - 1 - o.readEnd, seq->len - 1 - o.seqEnd ) ;
-					av = t4_overhang_align( pw + 4 * ( o.seqEnd + 1 ), r + o.readEnd + 1, R, bits + 32 * i + 16, ds ) ;
-				}
-				if ( av.dp )
-					t4_count( cx, 1, 1 ) ;
-				sstats[x] = t4_side_stats( av, !right ) ;
+				int x = base + cx.tid ;
+				bool p = x < 2 * overlapCnt && sstats[x].ind == -1 && !( easy && pre[x >> 1].hcCnt == 1 ) ;
+				unsigned m = __ballot_sync( T4_FULL, p ) ;
+				if ( p )
+					pend[cnt + __popc( m & ( ( 1u << cx.tid ) - 1u ) )] = x ;
+				cnt += __popc( m ) ;
 			}
-			T4_SYNC() ;
-			T4_PAR_FOR( i, overlapCnt )
-			{
-				if ( pre[i].hcCnt == 2 )
-					continue ;
-				T4Ovl e ;
-				int ok = t4_extend_finish( cx, len, t4_seq( cx, overlaps[i].seqIdx ), factor, overlaps[i], e, sstats[2 * i], sstats[2 * i + 1] ) ;
-				e.infoFromHits = ok ;
-				e.hcCnt = 2 ;
-				pre[i] = e ;
-			}
+			if ( cx.tid == 0 )
+				sm->bi[0] = cnt ;
+		}
+#else
+		{
+			int cnt = 0 ;
+			for ( int x = 0 ; x < 2 * overlapCnt ; ++x )
+				if ( sstats[x].ind == -1 && !( easy && pre[x >> 1].hcCnt == 1 ) )
+					pend[cnt++] = x ;
+			sm->bi[0] = cnt ;
+		}
+#endif
+		T4_SYNC() ;
+		c_overhang_dps( cx, overlaps, r, len, bits, pend, sm->bi[0], sstats ) ;
+		T4_PAR_FOR( i, overlapCnt )
+		{
+			if ( pre[i].hcCnt == 2 || sstats[2 * i].ind == -1 || sstats[2 * i + 1].ind == -1 )
+				continue ;
+			T4Ovl e ;
+			int ok = t4_extend_finish( cx, len, t4_seq( cx, overlaps[i].seqIdx ), factor, overlaps[i], e, sstats[2 * i], sstats[2 * i + 1] ) ;
+			e.infoFromHits = ok ;
+			e.hcCnt = 2 ;
+			pre[i] = e ;
 		}
 #if T4_CUDA
 		T4_SYNC() ;
