@@ -351,8 +351,25 @@ size_t t4_kmer_count_table_bytes(int64_t n_kmer_instances);
 int t4_kmer_count_stats_device(const void *read_pool, const void *qual_pool, const void *seq_off, const void *len, int64_t n,
                                int kmer_length, void *table, size_t table_bytes, void *min_cnt, void *median_cnt,
                                void *avg_cnt, void *new_len, void *cuda_stream);
-/* stats[0] k-mers counted, [1] distinct k-mers, [2] table slots, [3] 1 = table overflow (results invalid).  Synchronises. */
+/* stats[0] k-mers counted, [1] distinct k-mers, [2] table slots, [3] 1 = table overflow (results invalid), 2 = a barcode
+ * outside [0, barcode_max] (t4_barcode_kmer_count_stats_device; results invalid).  Synchronises. */
 int t4_kmer_count_table_stats(const void *table, size_t table_bytes, uint64_t stats[4]);
+/* The barcode-wise statistics of a --barcode run (main.cpp:1128-1180; threaded: BarcodeKmerCount_Thread, main.cpp:569-604):
+ * for every barcode a fresh KmerCount(21, 23) gets AddCount(read) of the reads of that barcode, then
+ * GetCountStatsAndTrim(read, NULL, barcodeMinCnt, barcodeMedianCnt, barcodeAvgCnt) for each of them (no quality trimming).
+ * bc_*[i] are read i's numbers, exactly as above but over its own barcode's reads only.  Reads may come in any order:
+ * one table keyed by (barcode, k-mer), one pass per 2^21 barcode ids that hold reads.  barcode[i] in [0, 2^31) (negative:
+ * T4_E_INVAL); kmer_length <= 21 (else T4_E_INVAL); reads longer than T4_MAX_READ_LEN: T4_E_UNSUPPORTED; a table
+ * overflow: T4_E_INTERNAL.  Host buffers; any output may be NULL.  Verified on an H100 against the reference. */
+int t4_barcode_kmer_count_stats(const char *read_pool, size_t pool_bytes, const uint64_t *seq_off, const int32_t *len,
+                                const int32_t *barcode, int64_t n, int kmer_length, int32_t *bc_min_cnt,
+                                int32_t *bc_median_cnt, float *bc_avg_cnt);
+/* The same on DEVICE buffers, asynchronous on cuda_stream: every barcode[i] must lie in [0, barcode_max] (one pass per
+ * 2^21 ids up to barcode_max, two launches of t4_kcount_bc_kernel each); `table` as for t4_kmer_count_stats_device.
+ * t4_kmer_count_table_stats afterwards tells whether the results are valid. */
+int t4_barcode_kmer_count_stats_device(const void *read_pool, const void *seq_off, const void *len, const void *barcode,
+                                       int64_t n, int32_t barcode_max, int kmer_length, void *table, size_t table_bytes,
+                                       void *bc_min_cnt, void *bc_median_cnt, void *bc_avg_cnt, void *cuda_stream);
 
 /* ---- stage-0 candidate extraction against a reference gene set (SURVEY.md 8f-4: fastq-extractor's predicate) --------
  * `SeqSet refSet(k); refSet.InputRefFa(fasta)` (FastqExtractor.cpp:313-318; SeqSet.hpp:2673-2864 with isIMGT == false:
@@ -395,6 +412,15 @@ int t4_refset_annotate(t4_refset *r, const char *read_pool, size_t pool_bytes, c
 int t4_sort_reads(const char *read_pool, size_t pool_bytes, const uint64_t *seq_off, const int32_t *len, const char *id_pool,
                   size_t id_pool_bytes, const uint64_t *id_off, const int32_t *min_cnt, const int32_t *median_cnt,
                   const float *avg_cnt, int64_t n, int64_t *order);
+/* The read order of a --barcode run: std::sort with CompReadWithBarcode (main.cpp:128-136: barcode ascending,
+ * barcodeMinCnt descending, then _sortRead::operator<).  The driver sorts by barcode while every barcodeMinCnt is still 0
+ * (main.cpp:1126), counts per barcode, then re-sorts each barcode group (main.cpp:1183-1192); one call after
+ * t4_barcode_kmer_count_stats gives the same sequence.  t4_sort_reads' arguments plus barcode[i] (>= 0: the comparator is
+ * an order only then; a negative one gives T4_E_INVAL) and barcode_min_cnt[i].  Verified on an H100 against the reference. */
+int t4_sort_reads_barcode(const char *read_pool, size_t pool_bytes, const uint64_t *seq_off, const int32_t *len,
+                          const char *id_pool, size_t id_pool_bytes, const uint64_t *id_off, const int32_t *min_cnt,
+                          const int32_t *median_cnt, const float *avg_cnt, const int32_t *barcode,
+                          const int32_t *barcode_min_cnt, int64_t n, int64_t *order);
 /* AlignAlgo::IsMateOverlap(fr, flen, sr, slen, minOverlap, offset, bestMatchCnt, checkTandem) (AlignAlgo.hpp:1027-1096)
  * for n read pairs, as ProcessRead calls it to detect read-through and overlapping mates (main.cpp:264, 291): overlap_size[i]
  * is the return value (-1: no unambiguous overlap), offset[i] / best_match_cnt[i] the two outputs as the function leaves them

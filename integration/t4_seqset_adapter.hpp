@@ -54,6 +54,8 @@
 #define t4_refset_annotate t4emu_refset_annotate
 #define t4_kmer_count_stats t4emu_kmer_count_stats
 #define t4_sort_reads t4emu_sort_reads
+#define t4_barcode_kmer_count_stats t4emu_barcode_kmer_count_stats
+#define t4_sort_reads_barcode t4emu_sort_reads_barcode
 #define t4_last_error t4emu_last_error
 #define t4_init t4emu_init
 #endif
@@ -608,6 +610,69 @@ public:
 		return true ;
 	}
 
+	// T4_BATCH_BARCODE_STATS() (opt-in, T4_BCSTATS=1) in front of `if (hasBarcode) { ... }` (main.cpp:1123-1194), which
+	// becomes the fall-back branch.  That block sorts the reads with CompReadWithBarcode (:1126), counts 21-mers per barcode
+	// group into barcodeMinCnt / barcodeMedianCnt / barcodeAvgCnt (:1128-1180), then re-sorts every barcode group with the
+	// same comparator (:1183-1192).  The first sort runs while every barcodeMinCnt is still 0 (the _sortRead constructor), so
+	// it only groups the reads by barcode, with operator< inside a group; the re-sort then orders each group by
+	// (barcodeMinCnt desc, operator<).  Together that is ONE sort of the whole list under CompReadWithBarcode with the final
+	// barcodeMinCnt, and the counting does not depend on the read order -- so the device counts first
+	// (t4_barcode_kmer_count_stats, reads in the driver's current order) and sorts once (t4_sort_reads_barcode).  With
+	// --barcode every read has a barcode >= 0 (main.cpp:797-819); the comparator is an order only then.  Not applicable --
+	// the CPU block runs -- without --barcode, with a negative barcode, or with a read over the device's length limit.
+	template <class Reads>
+	bool BatchBarcodeStats( Reads &sortedReads, int readCnt, bool hasBarcode )
+	{
+		const char *env = getenv( "T4_BCSTATS" ) ;
+		const int64_t n = readCnt ;
+		if ( !gpu || env == NULL || atoi( env ) != 1 || getenv( "T4_STREAMS" ) == NULL || !hasBarcode || n <= 0 || n != (int64_t)sortedReads.size() )
+			return false ;
+		std::string pool, idPool ;
+		std::vector<uint64_t> off( n ), idOff( n + 1 ) ;
+		std::vector<int32_t> len( n ), mn( n ), med( n ), bc( n ) ;
+		std::vector<float> avg( n ) ;
+		for ( int64_t i = 0 ; i < n ; ++i )
+		{
+			off[i] = pool.size() ;
+			len[i] = (int32_t)strlen( sortedReads[i].read ) ;
+			if ( len[i] > T4_MAX_READ_LEN || sortedReads[i].barcode < 0 )
+				return false ;
+			pool.append( sortedReads[i].read, len[i] ) ;
+			idOff[i] = idPool.size() ;
+			idPool.append( sortedReads[i].id ) ;
+			mn[i] = sortedReads[i].minCnt ; med[i] = sortedReads[i].medianCnt ; avg[i] = sortedReads[i].avgCnt ;
+			bc[i] = sortedReads[i].barcode ;
+		}
+		idOff[n] = idPool.size() ;
+		pool.append( 16, '\0' ) ;
+		idPool.append( 16, '\0' ) ;
+		std::vector<int32_t> bmn( n ), bmed( n ) ;
+		std::vector<float> bavg( n ) ;
+		Check( t4_barcode_kmer_count_stats( pool.data(), pool.size(), off.data(), len.data(), bc.data(), n, 21, bmn.data(), bmed.data(),
+			bavg.data() ) ) ;
+		for ( int64_t i = 0 ; i < n ; ++i )
+		{
+			sortedReads[i].barcodeMinCnt = bmn[i] ;
+			sortedReads[i].barcodeMedianCnt = bmed[i] ;
+			sortedReads[i].barcodeAvgCnt = bavg[i] ;
+		}
+		std::vector<int64_t> order( n ) ;
+		Check( t4_sort_reads_barcode( pool.data(), pool.size(), off.data(), len.data(), idPool.data(), idPool.size(), idOff.data(), mn.data(),
+			med.data(), avg.data(), bc.data(), bmn.data(), n, order.data() ) ) ;
+		Reads sorted ;
+		sorted.reserve( n ) ;
+		for ( int64_t j = 0 ; j < n ; ++j )
+			sorted.push_back( sortedReads[ order[j] ] ) ;
+		sortedReads.swap( sorted ) ;
+		int cells = 0 ;
+		for ( int64_t j = 0 ; j < n ; ++j )
+			if ( j == 0 || sortedReads[j].barcode != sortedReads[j - 1].barcode )
+				++cells ;
+		fprintf( stderr, "[trust4_b200] batch route: per-cell 21-mer statistics and barcode sort on the device, %lld reads in %d cells\n",
+			(long long)n, cells ) ;
+		return true ;
+	}
+
 	// main.cpp:674 `refSet.InputRefFa( optarg )`: the CPU object loads the genes as always; the file name is kept so that the
 	// batch route can build the same gene set on the device (BatchAnnotate).
 	void InputRefFa( char *filename, bool isIMGT = false, const char *imgtAdditionalGap = NULL )
@@ -841,6 +906,9 @@ public:
 
 // Opt-in (T4_KMERSTATS=1), in front of the count-statistics loop (main.cpp:981); see BatchKmerStats.
 #define T4_BATCH_KMERSTATS() if ( !seqSet.BatchKmerStats( sortedReads, readCnt, trimLevel, countMyself, contigMinCov > 0 ) )
+
+// Opt-in (T4_BCSTATS=1), in front of `if (hasBarcode)` (main.cpp:1123); see BatchBarcodeStats.
+#define T4_BATCH_BARCODE_STATS() if ( !seqSet.BatchBarcodeStats( sortedReads, readCnt, hasBarcode ) )
 
 // The third line (opt-in, T4_ANNOTATE=1), in front of the rough annotation loop (main.cpp:1084); see BatchAnnotate.
 #define T4_BATCH_ANNOTATE() if ( !seqSet.BatchAnnotate( sortedReads, refSet, readCnt ) )

@@ -38,6 +38,7 @@ EXPORTS = [
     "kmer_count_stats", "kmer_count_table_bytes", "kmer_count_stats_device", "kmer_count_table_stats",
     "refset_create_from_fa", "refset_free", "refset_size", "refset_name", "refset_seqset", "refset_set_hit_len_required",
     "refset_set_radius", "refset_scan", "refset_scan_device", "test_lis", "refset_get_overlaps", "refset_annotate", "sort_reads", "mate_overlap_batch",
+    "barcode_kmer_count_stats", "barcode_kmer_count_stats_device", "sort_reads_barcode",
 ]
 
 
@@ -137,6 +138,9 @@ class Lib:
         f("refset_annotate", ci, [vp, vp, C.c_size_t, vp, vp, C.c_int64, vp, vp])
         f("sort_reads", ci, [vp, C.c_size_t, vp, vp, vp, C.c_size_t, vp, vp, vp, vp, C.c_int64, vp])
         f("mate_overlap_batch", ci, [vp, C.c_size_t, vp, vp, vp, vp, vp, vp, C.c_int64, vp, vp, vp])
+        f("barcode_kmer_count_stats", ci, [vp, C.c_size_t, vp, vp, vp, C.c_int64, ci, vp, vp, vp])
+        f("barcode_kmer_count_stats_device", ci, [vp, vp, vp, vp, C.c_int64, C.c_int32, ci, vp, C.c_size_t, vp, vp, vp, vp])
+        f("sort_reads_barcode", ci, [vp, C.c_size_t, vp, vp, vp, C.c_size_t, vp, vp, vp, vp, vp, vp, C.c_int64, vp])
 
     def _f(self, name, restype, argtypes):
         fn = getattr(self.dll, self.prefix + name)
@@ -452,6 +456,24 @@ def kmer_count_stats(pool, seq_off, lens, k=21, lib: Lib | None = None, qual=Non
     return mn[:n], med[:n], avg[:n], nl[:n]
 
 
+def barcode_kmer_count_stats(pool, seq_off, lens, barcode, k=21, lib: Lib | None = None):
+    """t4_barcode_kmer_count_stats: (barcodeMinCnt, barcodeMedianCnt, barcodeAvgCnt) of every read, its k-mers counted
+    over the reads of its own barcode only (main.cpp:1128-1180).  Reads in any order; barcodes in [0, 2^31)."""
+    lib = lib or default_lib()
+    pool = np.ascontiguousarray(pool)
+    seq_off = np.ascontiguousarray(seq_off, dtype=np.uint64)
+    lens = np.ascontiguousarray(lens, dtype=np.int32)
+    barcode = np.ascontiguousarray(barcode, dtype=np.int32)
+    n = len(lens)
+    assert len(barcode) == n
+    mn = np.zeros(max(1, n), dtype=np.int32)
+    med = np.zeros(max(1, n), dtype=np.int32)
+    avg = np.zeros(max(1, n), dtype=np.float32)
+    lib.check(lib.barcode_kmer_count_stats(pool.ctypes.data, pool.nbytes, seq_off.ctypes.data, lens.ctypes.data, barcode.ctypes.data, n,
+                                           int(k), mn.ctypes.data, med.ctypes.data, avg.ctypes.data))
+    return mn[:n], med[:n], avg[:n]
+
+
 class RefSet:
     """Reference gene set on the device (t4_refset_create_from_fa: SeqSet::InputRefFa) and fastq-extractor's per-read
     predicate over it (t4_refset_scan: IsLowComplexity + SeqSet::HasHitInSet(read, 0))."""
@@ -535,6 +557,26 @@ def sort_reads(pool, seq_off, lens, ids, min_cnt, median_cnt, avg_cnt, lib: Lib 
                              id_off.ctypes.data, np.ascontiguousarray(min_cnt, dtype=np.int32).ctypes.data,
                              np.ascontiguousarray(median_cnt, dtype=np.int32).ctypes.data,
                              np.ascontiguousarray(avg_cnt, dtype=np.float32).ctypes.data, n, order.ctypes.data))
+    return order[:n]
+
+
+def sort_reads_barcode(pool, seq_off, lens, ids, min_cnt, median_cnt, avg_cnt, barcode, barcode_min_cnt, lib: Lib | None = None):
+    """t4_sort_reads_barcode: the permutation of std::sort(sortedReads, CompReadWithBarcode) (main.cpp:128-136) -- barcode
+    ascending, barcodeMinCnt descending, then sort_reads' order.  Barcodes must be >= 0."""
+    lib = lib or default_lib()
+    pool = np.ascontiguousarray(pool)
+    seq_off = np.ascontiguousarray(seq_off, dtype=np.uint64)
+    lens = np.ascontiguousarray(lens, dtype=np.int32)
+    n = len(lens)
+    idb = [i if isinstance(i, bytes) else i.encode() for i in ids]
+    id_off = np.zeros(n + 1, dtype=np.uint64)
+    id_off[1:] = np.cumsum([len(i) for i in idb])
+    id_pool = np.frombuffer(b"".join(idb) + b"\0" * 16, dtype=np.uint8).copy()
+    order = np.zeros(max(1, n), dtype=np.int64)
+    arrs = [np.ascontiguousarray(a, dtype=t) for a, t in ((min_cnt, np.int32), (median_cnt, np.int32), (avg_cnt, np.float32),
+                                                          (barcode, np.int32), (barcode_min_cnt, np.int32))]
+    lib.check(lib.sort_reads_barcode(pool.ctypes.data, pool.nbytes, seq_off.ctypes.data, lens.ctypes.data, id_pool.ctypes.data, id_pool.nbytes,
+                                     id_off.ctypes.data, *[a.ctypes.data for a in arrs], n, order.ctypes.data))
     return order[:n]
 
 

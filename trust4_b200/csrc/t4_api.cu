@@ -86,7 +86,14 @@ __global__ void __launch_bounds__( T4_MAX_NT, T4_MIN_BLOCKS ) t4_annot_kernel( c
 __global__ void t4_readsort_kernel( T4SortParams P )
 {
 	for ( i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x ; i < P.n ; i += (i64)gridDim.x * blockDim.x )
-		t4_sort_merge_one( P, i ) ;
+		t4_sort_merge_one<T4SortRec>( P, i ) ;
+}
+
+// the same pass in the --barcode order (CompReadWithBarcode)
+__global__ void t4_readsort_bc_kernel( T4SortParams P )
+{
+	for ( i64 i = (i64)blockIdx.x * blockDim.x + threadIdx.x ; i < P.n ; i += (i64)gridDim.x * blockDim.x )
+		t4_sort_merge_one<T4SortRecBc>( P, i ) ;
 }
 
 __global__ void t4_mate_overlap_kernel( T4MateParams P )
@@ -115,10 +122,25 @@ __global__ void __launch_bounds__( T4_MAX_NT ) t4_kcount_kernel( T4KcParams P, i
 	cx.sm = &sm[threadIdx.x / T4_KC_GROUP] ;
 	cx.tid = threadIdx.x % T4_KC_GROUP ;
 	cx.nt = T4_KC_GROUP ;
+	const T4KcBarcode B = { 0, 0, 0 } ;
 	if ( stats )
-		kc_stats_body( cx, P ) ;
+		kc_stats_body<false>( cx, P, B ) ;
 	else
-		kc_count_body( cx, P ) ;
+		kc_count_body<false>( cx, P, B ) ;
+}
+
+// the per-cell pass: one table keyed by (barcode, k-mer) for the barcodes of [B.lo, B.lo + 2^21)
+__global__ void __launch_bounds__( T4_MAX_NT ) t4_kcount_bc_kernel( T4KcParams P, int stats, T4KcBarcode B )
+{
+	__shared__ T4KcSmem sm[T4_MAX_NT / T4_KC_GROUP] ;
+	T4KcCtx cx ;
+	cx.sm = &sm[threadIdx.x / T4_KC_GROUP] ;
+	cx.tid = threadIdx.x % T4_KC_GROUP ;
+	cx.nt = T4_KC_GROUP ;
+	if ( stats )
+		kc_stats_body<true>( cx, P, B ) ;
+	else
+		kc_count_body<true>( cx, P, B ) ;
 }
 
 __global__ void t4_init_kernel( char *A, u64 base, T4InitParams ip )
@@ -2570,6 +2592,56 @@ int T4_API( refset_annotate )( t4_refset *r, const char *read_pool, size_t pool_
 // `std::sort( sortedReads.begin(), sortedReads.end() )` of the stage-1 driver (main.cpp:1078; _sortRead::operator<, :103-125):
 // order[j] = index of the record that comes j-th.  Host buffers; record i: read_pool[seq_off[i] .. + len[i]), its id
 // id_pool[id_off[i] .. id_off[i + 1]), its count statistics.  Verified on the GPU (t4_readsort.h).
+} // extern "C" (C++ helpers of the two sort entry points)
+static T4SortRec &sort_rec_base( T4SortRec &r ) { return r ; }
+static T4SortRec &sort_rec_base( T4SortRecBc &r ) { return r.r ; }
+
+// The merge sort of t4_sort_reads / t4_sort_reads_barcode over records the caller filled except for the read and id
+// fields (checked and set here); `kernel` is the merge pass of the record type.
+template <class Rec, class K> static int sort_records( const char *fn, K kernel, std::vector<Rec> &recs, const char *read_pool,
+	size_t pool_bytes, const uint64_t *seq_off, const int32_t *len, const char *id_pool, size_t id_pool_bytes, const uint64_t *id_off,
+	int64_t n, int64_t *order )
+{
+	std::vector<i64> idx( (size_t)n ) ;
+	for ( i64 i = 0 ; i < n ; ++i )
+	{
+		if ( len[i] < 0 || seq_off[i] + (u64)len[i] > pool_bytes || id_off[i + 1] < id_off[i] || id_off[i + 1] > id_pool_bytes )
+		{
+			set_err( std::string( fn ) + ": record outside its pool" ) ;
+			return T4_E_INVAL ;
+		}
+		T4SortRec &r = sort_rec_base( recs[(size_t)i] ) ;
+		r.len = len[i] ;
+		r.readOff = seq_off[i] ; r.idOff = id_off[i] ; r.idLen = (int32_t)( id_off[i + 1] - id_off[i] ) ; r.pad = 0 ;
+		idx[(size_t)i] = i ;
+	}
+	DevBuf m ;
+	Rec *dRec ;
+	char *dPool, *dId ;
+	i64 *from, *to ;
+	m.add( dRec, (size_t)n * sizeof( Rec ) ) ; m.add( dPool, pool_bytes + 16 ) ; m.add( dId, id_pool_bytes + 16 ) ; m.add( from, (size_t)n * 8 ) ;
+	m.add( to, (size_t)n * 8 ) ;
+	int rc = m.alloc() ;
+	if ( !rc ) rc = h2d( dRec, recs.data(), (size_t)n * sizeof( Rec ) ) ;
+	if ( !rc ) rc = h2d( dPool, read_pool, pool_bytes ) ;
+	if ( !rc ) rc = h2d( dId, id_pool, id_pool_bytes ) ;
+	if ( !rc ) rc = h2d( from, idx.data(), (size_t)n * 8 ) ;
+	T4SortParams P ;
+	memset( &P, 0, sizeof( P ) ) ;
+	P.recs = (u64)(uintptr_t)dRec ; P.pool = (u64)(uintptr_t)dPool ; P.idPool = (u64)(uintptr_t)dId ;
+	P.n = n ;
+	for ( i64 w = 1 ; !rc && w < n ; w *= 2 )
+	{
+		P.src = (u64)(uintptr_t)from ; P.dst = (u64)(uintptr_t)to ; P.width = w ;
+		rc = launch_items( kernel, P, n, 256 ) ;
+		i64 *t = from ; from = to ; to = t ;
+	}
+	if ( !rc ) rc = dsync() ;
+	if ( !rc ) rc = d2h( order, from, (size_t)n * 8 ) ;
+	return rc ;
+}
+extern "C" {
+
 int T4_API( sort_reads )( const char *read_pool, size_t pool_bytes, const uint64_t *seq_off, const int32_t *len, const char *id_pool,
 	size_t id_pool_bytes, const uint64_t *id_off, const int32_t *min_cnt, const int32_t *median_cnt, const float *avg_cnt, int64_t n,
 	int64_t *order )
@@ -2584,43 +2656,47 @@ int T4_API( sort_reads )( const char *read_pool, size_t pool_bytes, const uint64
 	if ( n == 0 )
 		return 0 ;
 	std::vector<T4SortRec> recs( (size_t)n ) ;
-	std::vector<i64> idx( (size_t)n ) ;
 	for ( i64 i = 0 ; i < n ; ++i )
 	{
-		if ( len[i] < 0 || seq_off[i] + (u64)len[i] > pool_bytes || id_off[i + 1] < id_off[i] || id_off[i + 1] > id_pool_bytes )
+		T4SortRec &r = recs[(size_t)i] ;
+		r.minCnt = min_cnt[i] ; r.medianCnt = median_cnt[i] ; r.avgCnt = avg_cnt[i] ;
+	}
+	return sort_records( "t4_sort_reads", T4_KERNEL( t4_readsort_kernel, t4_sort_merge_one<T4SortRec> ), recs, read_pool, pool_bytes, seq_off,
+		len, id_pool, id_pool_bytes, id_off, n, order ) ;
+}
+
+// `CompReadWithBarcode` order of a --barcode run (main.cpp:128-136): t4_sort_reads' records plus barcode[i] (>= 0) and
+// barcode_min_cnt[i].  One sort in this order, after the per-cell counts are known, is what the driver's two sorts
+// produce together (main.cpp:1126 while every barcodeMinCnt is still 0, i.e. grouped by barcode; then each barcode
+// group again at :1183-1192).  Host buffers; negative barcodes give T4_E_INVAL.  Verified on the GPU (t4_readsort.h).
+int T4_API( sort_reads_barcode )( const char *read_pool, size_t pool_bytes, const uint64_t *seq_off, const int32_t *len, const char *id_pool,
+	size_t id_pool_bytes, const uint64_t *id_off, const int32_t *min_cnt, const int32_t *median_cnt, const float *avg_cnt,
+	const int32_t *barcode, const int32_t *barcode_min_cnt, int64_t n, int64_t *order )
+{
+	int rc = ensure_up() ;
+	if ( rc ) return rc ;
+	if ( n < 0 || !read_pool || !seq_off || !len || !id_pool || !id_off || !min_cnt || !median_cnt || !avg_cnt || !barcode
+		|| !barcode_min_cnt || !order )
+	{
+		set_err( "t4_sort_reads_barcode: bad argument" ) ;
+		return T4_E_INVAL ;
+	}
+	std::vector<T4SortRecBc> recs( (size_t)n ) ;
+	for ( i64 i = 0 ; i < n ; ++i )
+	{
+		if ( barcode[i] < 0 )
 		{
-			set_err( "t4_sort_reads: record outside its pool" ) ;
+			set_err( "t4_sort_reads_barcode: negative barcode (CompReadWithBarcode is an order only on barcodes >= 0)" ) ;
 			return T4_E_INVAL ;
 		}
-		T4SortRec &r = recs[(size_t)i] ;
-		r.minCnt = min_cnt[i] ; r.medianCnt = median_cnt[i] ; r.avgCnt = avg_cnt[i] ; r.len = len[i] ;
-		r.readOff = seq_off[i] ; r.idOff = id_off[i] ; r.idLen = (int32_t)( id_off[i + 1] - id_off[i] ) ; r.pad = 0 ;
-		idx[(size_t)i] = i ;
+		T4SortRecBc &r = recs[(size_t)i] ;
+		r.r.minCnt = min_cnt[i] ; r.r.medianCnt = median_cnt[i] ; r.r.avgCnt = avg_cnt[i] ;
+		r.barcode = barcode[i] ; r.barcodeMinCnt = barcode_min_cnt[i] ;
 	}
-	DevBuf m ;
-	T4SortRec *dRec ;
-	char *dPool, *dId ;
-	i64 *from, *to ;
-	m.add( dRec, (size_t)n * sizeof( T4SortRec ) ) ; m.add( dPool, pool_bytes + 16 ) ; m.add( dId, id_pool_bytes + 16 ) ; m.add( from, (size_t)n * 8 ) ;
-	m.add( to, (size_t)n * 8 ) ;
-	rc = m.alloc() ;
-	if ( !rc ) rc = h2d( dRec, recs.data(), (size_t)n * sizeof( T4SortRec ) ) ;
-	if ( !rc ) rc = h2d( dPool, read_pool, pool_bytes ) ;
-	if ( !rc ) rc = h2d( dId, id_pool, id_pool_bytes ) ;
-	if ( !rc ) rc = h2d( from, idx.data(), (size_t)n * 8 ) ;
-	T4SortParams P ;
-	memset( &P, 0, sizeof( P ) ) ;
-	P.recs = (u64)(uintptr_t)dRec ; P.pool = (u64)(uintptr_t)dPool ; P.idPool = (u64)(uintptr_t)dId ;
-	P.n = n ;
-	for ( i64 w = 1 ; !rc && w < n ; w *= 2 )
-	{
-		P.src = (u64)(uintptr_t)from ; P.dst = (u64)(uintptr_t)to ; P.width = w ;
-		rc = launch_items( T4_KERNEL( t4_readsort_kernel, t4_sort_merge_one ), P, n, 256 ) ;
-		i64 *t = from ; from = to ; to = t ;
-	}
-	if ( !rc ) rc = dsync() ;
-	if ( !rc ) rc = d2h( order, from, (size_t)n * 8 ) ;
-	return rc ;
+	if ( n == 0 )
+		return 0 ;
+	return sort_records( "t4_sort_reads_barcode", T4_KERNEL( t4_readsort_bc_kernel, t4_sort_merge_one<T4SortRecBc> ), recs, read_pool,
+		pool_bytes, seq_off, len, id_pool, id_pool_bytes, id_off, n, order ) ;
 }
 
 // AlignAlgo::IsMateOverlap for n (first, second) read pairs of one pool (ProcessRead, main.cpp:264, 291): overlap_size[i] =
@@ -2685,21 +2761,30 @@ int T4_API( test_lis )( const int32_t *a, const int32_t *b, int n, int32_t *out_
 }
 
 // ---- canonical k-mer counts + per-read statistics (t4_kcount.h; SURVEY.md 8f-3) ------------------------------------
-static int kc_launch( const T4KcParams &P, int stats, void *stream )
+// B == NULL: the global table; else the per-cell pass over the barcodes of [B->lo, B->lo + 2^21)
+static int kc_launch( const T4KcParams &P, int stats, void *stream, const T4KcBarcode *B = NULL )
 {
 #if T4_CUDA
 	CK( cudaMemsetAsync( (void *)(uintptr_t)P.ctrl, 0, 8, (cudaStream_t)stream ) ) ; // the read cursor
-	t4_kcount_kernel<<<E.sms * 10, T4_MAX_NT, 0, (cudaStream_t)stream>>>( P, stats ) ; // 40 warps per SM (21 KB of shared memory per CTA)
+	if ( B ) // 40 warps per SM (21 KB of shared memory per CTA)
+		t4_kcount_bc_kernel<<<E.sms * 10, T4_MAX_NT, 0, (cudaStream_t)stream>>>( P, stats, *B ) ;
+	else
+		t4_kcount_kernel<<<E.sms * 10, T4_MAX_NT, 0, (cudaStream_t)stream>>>( P, stats ) ;
 	CK( cudaGetLastError() ) ;
 #else
 	*(u64 *)(uintptr_t)P.ctrl = 0 ;
 	T4KcSmem *sm = new T4KcSmem ;
 	T4KcCtx cx ;
 	cx.sm = sm ; cx.tid = 0 ; cx.nt = 1 ;
-	if ( stats )
-		kc_stats_body( cx, P ) ;
+	const T4KcBarcode none = { 0, 0, 0 } ;
+	if ( B && stats )
+		kc_stats_body<true>( cx, P, *B ) ;
+	else if ( B )
+		kc_count_body<true>( cx, P, *B ) ;
+	else if ( stats )
+		kc_stats_body<false>( cx, P, none ) ;
 	else
-		kc_count_body( cx, P ) ;
+		kc_count_body<false>( cx, P, none ) ;
 	delete sm ;
 #endif
 	return 0 ;
@@ -2811,6 +2896,141 @@ int T4_API( kmer_count_stats )( const char *read_pool, const char *qual_pool, si
 	if ( !r && median_cnt ) r = d2h( median_cnt, dMed, (size_t)n * 4 ) ;
 	if ( !r && avg_cnt ) r = d2h( avg_cnt, dAvg, (size_t)n * 4 ) ;
 	if ( !r && new_len ) r = d2h( new_len, dNew, (size_t)n * 4 ) ;
+	return r ;
+}
+
+// The per-cell passes of the device form: one count + statistics launch pair per barcode range of 2^21 ids in `ranges`
+// (range j = barcodes [j << 21, (j + 1) << 21)).  The table is cleared before each pass; ctrl[1..3] add up over the passes.
+static int bc_kc_passes( T4KcParams &P, const void *barcode, int barcode_max, const std::vector<int> &ranges, void *stream )
+{
+	int r = 0 ;
+	T4KcBarcode B ;
+	B.barcode = (u64)(uintptr_t)barcode ;
+	B.max = barcode_max ;
+	for ( size_t j = 0 ; !r && j < ranges.size() ; ++j )
+	{
+		B.lo = ranges[j] << T4_KC_BC_BITS ;
+		r = dzero( (void *)(uintptr_t)P.keys, P.cap * 12, stream ) ; // keys and counts; ctrl keeps the totals
+		if ( !r ) r = kc_launch( P, 0, stream, &B ) ;
+		if ( !r ) r = kc_launch( P, 1, stream, &B ) ;
+	}
+	return r ;
+}
+
+static void kc_params( T4KcParams &P, void *table, size_t table_bytes, const void *pool, const void *seq_off, const void *len, int64_t n,
+	int k, void *min_cnt, void *median_cnt, void *avg_cnt )
+{
+	u64 cap = 1024 ;
+	while ( cap * 2 * 12 + 256 <= table_bytes )
+		cap <<= 1 ;
+	memset( &P, 0, sizeof( P ) ) ;
+	char *t = (char *)table ;
+	P.keys = (u64)(uintptr_t)t ;
+	P.counts = (u64)(uintptr_t)( t + cap * 8 ) ;
+	P.ctrl = (u64)(uintptr_t)( t + cap * 12 ) ;
+	P.cap = cap ;
+	P.pool = (u64)(uintptr_t)pool ;
+	P.seqOff = (u64)(uintptr_t)seq_off ;
+	P.len = (u64)(uintptr_t)len ;
+	P.minCnt = (u64)(uintptr_t)min_cnt ;
+	P.medianCnt = (u64)(uintptr_t)median_cnt ;
+	P.avgCnt = (u64)(uintptr_t)avg_cnt ;
+	P.n = n ;
+	P.k = k ;
+}
+
+// Device-pointer form of the per-cell statistics: `pool`, `seq_off` (u64[n]), `len` (i32[n]), `barcode` (i32[n], every
+// id in [0, barcode_max]) and the outputs are DEVICE buffers, `table` a device buffer of t4_kmer_count_table_bytes()
+// bytes.  Runs one pass per 2^21 barcode ids up to barcode_max.  Asynchronous on cuda_stream; t4_kmer_count_table_stats
+// then reports the totals and whether the results are invalid (stats[3] = 1 table overflow, 2 a barcode outside
+// [0, barcode_max]).
+int T4_API( barcode_kmer_count_stats_device )( const void *pool, const void *seq_off, const void *len, const void *barcode, int64_t n,
+	int32_t barcode_max, int kmer_length, void *table, size_t table_bytes, void *min_cnt, void *median_cnt, void *avg_cnt, void *cuda_stream )
+{
+	int r = ensure_up() ;
+	if ( r ) return r ;
+	if ( n < 0 || barcode_max < 0 || kmer_length < 2 || kmer_length > 21 || table_bytes < 1024 * 12 + 256 )
+	{
+		set_err( "t4_barcode_kmer_count_stats: bad argument" ) ;
+		return T4_E_INVAL ;
+	}
+	T4KcParams P ;
+	kc_params( P, table, table_bytes, pool, seq_off, len, n, kmer_length, min_cnt, median_cnt, avg_cnt ) ;
+	std::vector<int> ranges ;
+	for ( int j = 0 ; j <= ( barcode_max >> T4_KC_BC_BITS ) ; ++j )
+		ranges.push_back( j ) ;
+	r = dzero( table, P.cap * 12 + 64, cuda_stream ) ;
+	if ( !r ) r = bc_kc_passes( P, barcode, barcode_max, ranges, cuda_stream ) ;
+	return r ;
+}
+
+// The barcode-wise statistics of a --barcode run (main.cpp:1128-1180, BarcodeKmerCount_Thread :569-604): for every
+// barcode, KmerCount( kmer_length ) over the reads of that barcode only, then GetCountStatsAndTrim( read, NULL, ... )
+// into bc_min_cnt / bc_median_cnt / bc_avg_cnt.  Reads may come in any order.  Host buffers; barcode ids in [0, 2^31);
+// negative ones and kmer_length > 21 give T4_E_INVAL, reads longer than T4_MAX_READ_LEN T4_E_UNSUPPORTED.
+int T4_API( barcode_kmer_count_stats )( const char *read_pool, size_t pool_bytes, const uint64_t *seq_off, const int32_t *len,
+	const int32_t *barcode, int64_t n, int kmer_length, int32_t *bc_min_cnt, int32_t *bc_median_cnt, float *bc_avg_cnt )
+{
+	int r = ensure_up() ;
+	if ( r ) return r ;
+	if ( n < 0 || !read_pool || !seq_off || !len || !barcode || kmer_length < 2 || kmer_length > 21 )
+	{
+		set_err( "t4_barcode_kmer_count_stats: bad argument" ) ;
+		return T4_E_INVAL ;
+	}
+	r = check_records( "t4_barcode_kmer_count_stats", pool_bytes, seq_off, len, n ) ;
+	if ( r || n == 0 )
+		return r ;
+	u64 inst = 0 ;
+	int bmax = 0 ;
+	std::vector<char> present ;
+	for ( i64 i = 0 ; i < n ; ++i )
+	{
+		if ( barcode[i] < 0 )
+		{
+			set_err( "t4_barcode_kmer_count_stats: negative barcode" ) ;
+			return T4_E_INVAL ;
+		}
+		const int j = barcode[i] >> T4_KC_BC_BITS ;
+		if ( j >= (int)present.size() )
+			present.resize( j + 1, 0 ) ;
+		present[j] = 1 ;
+		if ( barcode[i] > bmax )
+			bmax = barcode[i] ;
+		if ( len[i] >= kmer_length )
+			inst += (u64)( len[i] - kmer_length + 1 ) ;
+	}
+	std::vector<int> ranges ; // only the ranges that hold reads
+	for ( int j = 0 ; j < (int)present.size() ; ++j )
+		if ( present[j] )
+			ranges.push_back( j ) ;
+	const size_t tb = T4_API( kmer_count_table_bytes )( (int64_t)inst ) ;
+	DevBuf m ;
+	char *dPool, *dTab ;
+	u64 *dOff ;
+	int32_t *dLen, *dBc, *dMin, *dMed ;
+	float *dAvg ;
+	m.add( dPool, pool_bytes + 16 ) ; m.add( dOff, (size_t)n * 8 ) ; m.add( dLen, (size_t)n * 4 ) ; m.add( dBc, (size_t)n * 4 ) ;
+	m.add( dMin, (size_t)n * 4 ) ; m.add( dMed, (size_t)n * 4 ) ; m.add( dAvg, (size_t)n * 4 ) ; m.add( dTab, tb ) ;
+	r = m.alloc() ;
+	if ( !r ) r = h2d( dPool, read_pool, pool_bytes ) ;
+	if ( !r ) r = h2d( dOff, seq_off, (size_t)n * 8 ) ;
+	if ( !r ) r = h2d( dLen, len, (size_t)n * 4 ) ;
+	if ( !r ) r = h2d( dBc, barcode, (size_t)n * 4 ) ;
+	T4KcParams P ;
+	kc_params( P, dTab, tb, dPool, dOff, dLen, n, kmer_length, dMin, dMed, dAvg ) ;
+	if ( !r ) r = dzero( dTab, P.cap * 12 + 64 ) ;
+	if ( !r ) r = bc_kc_passes( P, dBc, bmax, ranges, 0 ) ;
+	u64 st[4] = { 0, 0, 0, 0 } ;
+	if ( !r ) r = T4_API( kmer_count_table_stats )( dTab, tb, st ) ;
+	if ( !r && st[3] )
+	{
+		set_err( st[3] == 1 ? "t4_barcode_kmer_count_stats: count table overflow" : "t4_barcode_kmer_count_stats: barcode out of range" ) ;
+		r = T4_E_INTERNAL ;
+	}
+	if ( !r && bc_min_cnt ) r = d2h( bc_min_cnt, dMin, (size_t)n * 4 ) ;
+	if ( !r && bc_median_cnt ) r = d2h( bc_median_cnt, dMed, (size_t)n * 4 ) ;
+	if ( !r && bc_avg_cnt ) r = d2h( bc_avg_cnt, dAvg, (size_t)n * 4 ) ;
 	return r ;
 }
 

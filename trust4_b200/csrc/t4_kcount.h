@@ -20,6 +20,15 @@
 //          (scan over the lanes), the median is found by rank counting (the element with exactly m/2 smaller-or-earlier
 //          elements is c[m/2] of the sorted array), min and sum by a group reduction; the trimming and the N rules of
 //          KmerCount.hpp:241-283 follow.
+//
+// Per-cell variant (BC = true; the barcode-wise count of --barcode runs, main.cpp:1128-1180): the reference gives every
+// barcode group a fresh KmerCount( 21, 23 ) (Clear() between groups), AddCount over the group, then
+// GetCountStatsAndTrim( read, NULL, ... ).  Clearing a table per barcode is the same as keying one table by (barcode,
+// canonical k-mer): key = code + 1 in the low 43 bits (k <= 21) and barcode - lo above them, so one count launch and one
+// statistics launch cover every barcode of [lo, lo + 2^21) in any read order; the host runs one pass per such range that
+// holds reads (barcode ids up to 2^31 - 1 stay exact; nothing is hashed into fewer bits).  The slot hash mixes all 64 key
+// bits: the global hash only sees the key's low bits, so the same k-mer of many cells would share one probe chain.
+// The global pass (BC = false) is the same code with these parts compiled out.
 #ifndef T4_KCOUNT_H
 #define T4_KCOUNT_H
 
@@ -43,6 +52,16 @@ struct T4KcParams
 	int pad ;
 } ;
 
+// the barcode of the per-cell pass (a parameter of its own: T4KcParams and the global kernel keep their layout)
+struct T4KcBarcode
+{
+	u64 barcode ;          // i32[n] barcode id of every read
+	int lo ;               // this pass counts the reads with lo <= barcode < lo + 2^T4_KC_BC_BITS
+	int max ;              // the largest valid barcode id: a read outside [0, max] flags ctrl[3] = 2 (results invalid)
+} ;
+
+#define T4_KC_BC_SHIFT 43          /* key bits of code + 1 (k <= 21: code < 2^42) */
+#define T4_KC_BC_BITS 21           /* barcode bits of a key: barcode - lo < 2^21 */
 #define T4_KC_MAX_POS T4_DEV_MAX_READ
 #define T4_KC_MAX_PROBES 4096      /* linear-probe bound: at load <= 1/2 clusters are a few slots long; beyond this the table is treated as full */
 #define T4_KC_GROUP 32             /* threads that share a read: one warp (a CTA of 128 per read spent its time at CTA barriers and
@@ -60,6 +79,35 @@ struct T4KcSmem                    // per group (warp)
 } ;
 
 T4_HD inline u64 t4_kc_hash( u64 key, u64 cap ) { return ( ( key * 0x9E3779B97F4A7C15ull ) >> 20 ) & ( cap - 1 ) ; }
+
+// per-cell keys: a full 64-bit mix (the splitmix64 finaliser), so that the barcode bits move the slot
+T4_HD inline u64 t4_kc_hash_bc( u64 key, u64 cap )
+{
+	key ^= key >> 33 ;
+	key *= 0xFF51AFD7ED558CCDull ;
+	key ^= key >> 33 ;
+	key *= 0xC4CEB9FE1A85EC53ull ;
+	key ^= key >> 33 ;
+	return key & ( cap - 1 ) ;
+}
+
+// the key bits above the k-mer for read r: false = the read is not counted in this pass (BC only)
+template <bool BC> T4_D inline bool kc_read_key( const T4KcParams &P, const T4KcBarcode &B, i64 r, u64 &hi )
+{
+	hi = 0 ;
+	if ( !BC )
+		return true ;
+	const int b = t4_x<int32_t>( B.barcode )[r] ;
+	if ( b < 0 || b > B.max )
+	{
+		t4_x<u64>( P.ctrl )[3] = 2 ;
+		return false ;
+	}
+	if ( b < B.lo || b - B.lo >= ( 1 << T4_KC_BC_BITS ) )
+		return false ;
+	hi = (u64)( b - B.lo ) << T4_KC_BC_SHIFT ;
+	return true ;
+}
 
 // nucToNum[ c - 'A' ] & 3 (main.cpp:39-42) with N kept apart; selects, no branches
 T4_HD inline unsigned char t4_kc_code( char c )
@@ -139,8 +187,8 @@ T4_D inline void kc_load_read( T4KcCtx &cx, const T4KcParams &P, i64 r, int len 
 	T4_KC_SYNC() ;
 }
 
-// KmerCount::AddCount for the reads this group draws
-T4_D inline void kc_count_body( T4KcCtx &cx, const T4KcParams &P )
+// KmerCount::AddCount for the reads this group draws (BC: into the table of the read's barcode)
+template <bool BC> T4_D inline void kc_count_body( T4KcCtx &cx, const T4KcParams &P, const T4KcBarcode &B )
 {
 	u64 *keys = t4_x<u64>( P.keys ) ;
 	u32 *counts = t4_x<u32>( P.counts ) ;
@@ -149,6 +197,9 @@ T4_D inline void kc_count_body( T4KcCtx &cx, const T4KcParams &P )
 	for ( i64 r0 = kc_next_batch( cx, P ) ; r0 >= 0 ; r0 = kc_next_batch( cx, P ) )
 	for ( i64 r = r0 ; r < r0 + T4_KC_BATCH && r < P.n ; ++r )
 	{
+		u64 hi ;
+		if ( !kc_read_key<BC>( P, B, r, hi ) )
+			continue ;
 		const int len = t4_x<int32_t>( P.len )[r] ;
 		if ( len < P.k || len > T4_DEV_MAX_READ )
 			continue ;
@@ -167,8 +218,8 @@ T4_D inline void kc_count_body( T4KcCtx &cx, const T4KcParams &P )
 			u64 code ;
 			if ( !t4_kc_roll_step( R, cx.sm->code, q, P.k, &code ) )
 				continue ;
-			const u64 key = code + 1 ;
-			u64 s = t4_kc_hash( key, P.cap ) ;
+			const u64 key = BC ? ( code + 1 ) | hi : code + 1 ;
+			u64 s = BC ? t4_kc_hash_bc( key, P.cap ) : t4_kc_hash( key, P.cap ) ;
 			u64 probes = 0 ;
 			while ( 1 )
 			{
@@ -203,11 +254,11 @@ T4_D inline void kc_count_body( T4KcCtx &cx, const T4KcParams &P )
 		t4_atomic_add( ctrl + 2, fresh ) ;
 }
 
-T4_D inline u32 kc_lookup( const T4KcParams &P, u64 code )
+template <bool BC> T4_D inline u32 kc_lookup( const T4KcParams &P, u64 code, u64 hi )
 {
 	const u64 *keys = t4_x<u64>( P.keys ) ;
-	const u64 key = code + 1 ;
-	u64 s = t4_kc_hash( key, P.cap ) ;
+	const u64 key = BC ? ( code + 1 ) | hi : code + 1 ;
+	u64 s = BC ? t4_kc_hash_bc( key, P.cap ) : t4_kc_hash( key, P.cap ) ;
 	for ( int probes = 0 ; probes <= T4_KC_MAX_PROBES ; ++probes ) // bounded like the insert: an overfull table cannot hang the launch
 	{
 		const u64 cur = keys[s] ;
@@ -239,8 +290,9 @@ T4_D inline u32 kc_scan( T4KcCtx &cx, u32 v, u32 &total )
 	return base ;
 }
 
-// KmerCount::GetCountStatsAndTrim( read, qual, ... ) for the reads this group draws
-T4_D inline void kc_stats_body( T4KcCtx &cx, const T4KcParams &P )
+// KmerCount::GetCountStatsAndTrim( read, qual, ... ) for the reads this group draws (BC: qual is 0; the reads of other
+// passes are left alone)
+template <bool BC> T4_D inline void kc_stats_body( T4KcCtx &cx, const T4KcParams &P, const T4KcBarcode &B )
 {
 	T4KcSmem *sm = cx.sm ;
 	int32_t *minCnt = t4_x<int32_t>( P.minCnt ), *medianCnt = t4_x<int32_t>( P.medianCnt ) ;
@@ -248,6 +300,9 @@ T4_D inline void kc_stats_body( T4KcCtx &cx, const T4KcParams &P )
 	for ( i64 r0 = kc_next_batch( cx, P ) ; r0 >= 0 ; r0 = kc_next_batch( cx, P ) )
 	for ( i64 r = r0 ; r < r0 + T4_KC_BATCH && r < P.n ; ++r )
 	{
+		u64 hi ;
+		if ( !kc_read_key<BC>( P, B, r, hi ) )
+			continue ;
 		const int len = t4_x<int32_t>( P.len )[r] ;
 		if ( len < P.k || len > T4_DEV_MAX_READ )
 		{
@@ -277,7 +332,7 @@ T4_D inline void kc_stats_body( T4KcCtx &cx, const T4KcParams &P )
 			u64 code ;
 			if ( t4_kc_roll_step( R, sm->code, q, P.k, &code ) )
 			{
-				int c = (int)kc_lookup( P, code ) ;
+				int c = (int)kc_lookup<BC>( P, code, hi ) ;
 				if ( c <= 0 )
 					c = 1 ; // KmerCount.hpp:222-223
 				sm->valid[q] = (u32)c ;

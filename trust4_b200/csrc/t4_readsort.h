@@ -9,7 +9,8 @@
 //
 // STATUS: verified on an H100 (tests/test_gpu_preprocess.py) against the reference's std::sort and, at 2^20 + 3 records
 // (more than one grid of the grid-stride loop), against a Python restatement of the comparator; a kernel of its own
-// (t4_readsort_kernel).
+// (t4_readsort_kernel).  The --barcode order (CompReadWithBarcode, T4SortRecBc below) is the same merge body over a wider
+// record (t4_readsort_bc_kernel), verified the same way (tests/test_gpu_barcode_stats.py).
 #ifndef T4_READSORT_H
 #define T4_READSORT_H
 
@@ -65,10 +66,30 @@ T4_HD inline bool t4_sortrec_less( const T4SortRec &a, const T4SortRec &b, const
 	return t4_strcmp_n( idPool + a.idOff, a.idLen, idPool + b.idOff, b.idLen ) < 0 ;
 }
 
-// output position of src[i] in the merge of its pair of runs
-T4_HD inline void t4_sort_merge_one( const T4SortParams &P, i64 i )
+// The record of the --barcode order: `CompReadWithBarcode` (main.cpp:128-136) -- barcode ascending, barcodeMinCnt
+// descending, then _sortRead::operator<.  A record of its own, so that the global sort keeps its record and its kernel.
+// The reference's comparator special-cases barcode -1 and is a strict weak order only when every barcode is >= 0 (with
+// --barcode every read has one, main.cpp:797-819); the entry point rejects negative barcodes, and for barcodes >= 0 the
+// comparison below is the reference's.
+struct T4SortRecBc
 {
-	const T4SortRec *recs = t4_x<T4SortRec>( P.recs ) ;
+	T4SortRec r ;
+	int32_t barcode, barcodeMinCnt ;
+} ;
+
+T4_HD inline bool t4_sortrec_less( const T4SortRecBc &a, const T4SortRecBc &b, const char *pool, const char *idPool )
+{
+	if ( a.barcode != b.barcode )
+		return a.barcode < b.barcode ;
+	else if ( a.barcodeMinCnt != b.barcodeMinCnt )
+		return a.barcodeMinCnt > b.barcodeMinCnt ;
+	return t4_sortrec_less( a.r, b.r, pool, idPool ) ;
+}
+
+// output position of src[i] in the merge of its pair of runs (Rec: T4SortRec or T4SortRecBc)
+template <class Rec> T4_HD inline void t4_sort_merge_one( const T4SortParams &P, i64 i )
+{
+	const Rec *recs = t4_x<Rec>( P.recs ) ;
 	const char *pool = t4_x<char>( P.pool ), *idPool = t4_x<char>( P.idPool ) ;
 	const i64 *src = t4_x<i64>( P.src ) ;
 	i64 *dst = t4_x<i64>( P.dst ) ;
@@ -76,7 +97,7 @@ T4_HD inline void t4_sort_merge_one( const T4SortParams &P, i64 i )
 	const i64 base = ( i / ( 2 * w ) ) * ( 2 * w ) ;
 	const i64 aEnd = base + w < P.n ? base + w : P.n ;
 	const i64 bEnd = base + 2 * w < P.n ? base + 2 * w : P.n ;
-	const T4SortRec &x = recs[ src[i] ] ;
+	const Rec &x = recs[ src[i] ] ;
 	if ( i < aEnd )
 	{
 		// left run: count the right run's elements that come strictly before x
