@@ -66,7 +66,11 @@ void t4_seqset_destroy(t4_seqset *s);
 int t4_seqset_set_hit_len_required(t4_seqset *s, int l);
 /* SeqSet::SetNovelSeqSimilarity, SeqSet.hpp:2606 */
 int t4_seqset_set_novel_seq_similarity(t4_seqset *s, double v);
-/* SeqSet::SetConsiderBarcodeInIndexHash, SeqSet.hpp:2611 */
+/* SeqSet::SetConsiderBarcodeInIndexHash, SeqSet.hpp:2611.  As in the reference's KmerIndex (bucket
+ * (code + barcode + 1) % 1000003, KmerIndex.hpp:29-33), two barcodes share one postings list per k-mer exactly when
+ * barcode + 1 is equal modulo 1000003 (5 and 1000008; -1, i.e. no barcode, and 1000002): the >= 100-postings skip rule
+ * of GetHitsFromRead sees the shared list's size, and a read without a barcode gets the hits on 1000002's contigs.
+ * Needs k <= 15. */
 int t4_seqset_set_consider_barcode_in_hash(t4_seqset *s, int on);
 /* SeqSet::SetIsLongSeqSet, SeqSet.hpp:11082 -- only `0` is supported (reads <= 200 bp). */
 int t4_seqset_set_is_long(t4_seqset *s, int on);

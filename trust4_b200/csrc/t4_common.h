@@ -41,6 +41,7 @@ typedef int64_t i64;
 #define T4_DEV_MAX_READ T4_MAX_READ_LEN       /* device-side read length limit (reads > 200 bp make the reference switch to isLongSeqSet) */
 #define T4_ALIGN 32               /* arena allocations are sector aligned: a postings list of <= 4 entries is ONE 32-byte sector */
 #define T4_BIG_REPEAT 10000       /* SeqSet.hpp:799, 875, 937: hits[k].repeats <= 10000 */
+#define T4_KINDEX_HASH_MAX 1000003u /* KmerIndex.hpp:21: buckets of the k-mer index; barcodes equal modulo it share postings lists */
 
 // ---- key layout of a seed hit (one u64 per hit; SeqSet.hpp:53 `_hit` carries the same information) ----
 // [63] strand (+1 -> 1, -1 -> 0) | [62:41] contig slot | [40:20] diagonal c = a - b + 2^20 | [19:1] contig offset b | [0] repeats > 10000

@@ -253,11 +253,13 @@ T4_HD inline int t4_key_big( u64 k ) { return (int)( k & 1 ) ; }
 // ---------------------------------------------------------------------------
 T4_D inline u64 t4_index_key( T4Stream *st, u64 code, int barcode )
 {
-	// KmerIndex::GetHash salts the bucket with barcode + 1 when considerBarcode is set (KmerIndex.hpp:29-33);
-	// the postings lists are then effectively per (k-mer, barcode).
+	// KmerIndex::GetHash salts the bucket with barcode + 1 when considerBarcode is set (KmerIndex.hpp:29-33): bucket
+	// (code + barcode + 1) % 1000003, and inside the bucket the map key is the code alone.  So one postings list serves
+	// every barcode of one residue (barcode + 1) % 1000003: barcodes 5 and 1000008 share their lists, barcode -1 shares
+	// with 1000002.  The salt is that residue; the barcode filter of GetHitsFromRead drops the foreign postings.
 	u64 key = code ;
 	if ( st->considerBarcode )
-		key += (u64)(u32)( barcode + 1 ) << ( 2 * st->kmerLength ) ;
+		key += (u64)( (u32)( barcode + 1 ) % T4_KINDEX_HASH_MAX ) << ( 2 * st->kmerLength ) ;
 	return key + 1 ;
 }
 

@@ -538,7 +538,7 @@ __global__ void __launch_bounds__( 32 * T4P_WARPS, MINB ) t4_probe_kernel( T4Pro
 		R.nPos = 2 * R.m ;
 		R.dir = (const T4Dir *)( P.A + st->dirOff ) ;
 		R.dirMask = st->dirCap - 1 ;
-		R.salt = st->considerBarcode ? ( (u64)(u32)( R.barcode + 1 ) << ( 2 * R.k ) ) : 0ull ;
+		R.salt = st->considerBarcode ? ( (u64)( (u32)( R.barcode + 1 ) % T4_KINDEX_HASH_MAX ) << ( 2 * R.k ) ) : 0ull ;
 		R.mask = ( 1ull << ( 2 * R.k ) ) - 1ull ; // k <= 31
 		if ( R.len > T4_DEV_MAX_READ || R.len < R.k )
 		{
