@@ -269,13 +269,16 @@ int t4_streams_error(t4_seqset *const *sets, int n_sets);
 int t4_streams_cycles(t4_seqset *const *sets, int n_sets, uint64_t *cycles);
 /* Test hook: number of postings in the k-mer index and an order-independent checksum of them. */
 int64_t t4_seqset_index_checksum(t4_seqset *s, uint64_t *checksum);
+/* Test hook: checks the equality byte the engine keeps beside every posWeight column of every live contig against the
+ * column; returns the number of columns checked, *bad the number whose byte is not IsBaseEqual of the column. */
+int64_t t4_test_check_eq_bytes(t4_seqset *s, int64_t *bad);
 
 /* Device counters accumulated since the last t4_reset()/probe (summed over streams):
  * [0] reads processed, [1] overhang DPs (ExtendOverlap), [2] k-mer lookups executed, [3] postings read (sum c_j),
  * [4] hits emitted (sum c_j'), [5] packed read bytes ceil(L/4), [6] overlaps scored, [7] gap DPs,
  * [8..15] clock cycles per phase: other, probe, hit sort, chains, scoring, ExtendOverlap, decide+commit,
- * InputNovelRead/RepeatAddRead/consensus; [16] overlaps extended; [17..19] cycles inside ExtendOverlap (bit masks,
- * classification, DPs), [20] reads taking the lazy ExtendOverlap path; [21] ExtendOverlaps the decision loop still runs
+ * InputNovelRead/RepeatAddRead/consensus; [16] overlaps extended; [17..19] cycles inside ExtendOverlap (bit masks with
+ * the settling of every side that needs no DP, the list of deferred sides, their DPs), [20] reads taking the lazy ExtendOverlap path; [21] ExtendOverlaps the decision loop still runs
  * on demand on its single thread (s_make_exact: overlaps it consults without a result), [22] the clock cycles they take;
  * [23] reserved. */
 #define T4_N_COUNTERS 24

@@ -37,7 +37,7 @@ EXPORTS = [
     "streams_assign_reads", "assign_free", "assign_results", "assign_stats", "assign_extended_set", "assign_device_buffers",
     "kmer_count_stats", "kmer_count_table_bytes", "kmer_count_stats_device", "kmer_count_table_stats",
     "refset_create_from_fa", "refset_free", "refset_size", "refset_name", "refset_seqset", "refset_set_hit_len_required",
-    "refset_set_radius", "refset_scan", "refset_scan_device", "test_lis", "refset_get_overlaps", "refset_annotate", "sort_reads", "mate_overlap_batch",
+    "refset_set_radius", "refset_scan", "refset_scan_device", "test_lis", "test_check_eq_bytes", "refset_get_overlaps", "refset_annotate", "sort_reads", "mate_overlap_batch",
     "barcode_kmer_count_stats", "barcode_kmer_count_stats_device", "sort_reads_barcode",
 ]
 
@@ -267,6 +267,17 @@ class SeqSet:
         if n < 0:
             return n, None, None
         return n, out[:n], sim[:n]
+
+    def check_eq_bytes(self):
+        """(columns checked, columns whose equality byte disagrees with their posWeight counts) over every live contig."""
+        if not hasattr(self.lib, "test_check_eq_bytes"):
+            # resolved on first use, so that a build from before the cache (bench/ab_compare.py's parent) still loads
+            self.lib._f("test_check_eq_bytes", C.c_int64, [C.c_void_p, C.POINTER(C.c_int64)])
+        bad = C.c_int64(0)
+        n = self.lib.test_check_eq_bytes(self.h, C.byref(bad))
+        if n < 0:
+            self.lib.check(int(n))
+        return int(n), int(bad.value)
 
     def index_checksum(self):
         cs = C.c_uint64()

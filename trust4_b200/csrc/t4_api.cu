@@ -170,10 +170,11 @@ __global__ void t4_pack_kernel( char *A, const u64 *streamOff, const u64 *outOff
 // variant 2 = w_side_pair (ExtendOverlap's overhang pass: problems 2k and 2k+1 on the two halves of warp k, as a left
 //             side, scanned from its end, and a right side); writes each problem's T4SideStats, not its edit string.
 // One warp per problem (variant 2: per pair).  scratch: per problem 13 * actStride u32 traceback words + an edit-string
-// buffer (large n).
+// buffer (large n).  The problems come as posWeight columns; the kernel derives their equality bytes (t4_eq) itself.
 __global__ void t4_dp_hot_kernel( int n, int variant, const int *tw, const i64 *off, const char *p, signed char *align, const i64 *alignOff,
 	int *score, u32 *scratch, const i64 *scratchOff )
 {
+	__shared__ unsigned char eqb[2][T4_DEV_MAX_READ] ;
 	__shared__ u32 nib[2][64] ;
 	__shared__ u32 bits[2][16] ;
 	__shared__ u32 act[2][13 * T4_WACT_WORDS] ;
@@ -189,7 +190,9 @@ __global__ void t4_dp_hot_kernel( int n, int variant, const int *tw, const i64 *
 			const int k = 2 * blockIdx.x + h ;
 			T4DpSide &d = s[h] ;
 			d.n = ( k < n ) ? (int)( off[k + 1] - off[k] ) : 0 ;
-			d.tw = tw + 4 * off[k < n ? k : 0] ;
+			for ( int t = threadIdx.x ; t < d.n ; t += 32 )
+				eqb[h][t] = (unsigned char)t4_eq_nibble( tw + 4 * ( off[k] + t ) ) ;
+			d.te = eqb[h] ;
 			d.p = p + off[k < n ? k : 0] ;
 			d.fromEnd = ( h == 0 ) ;
 			const bool small = d.n < 16 * T4_WACT_WORDS ;
@@ -198,6 +201,7 @@ __global__ void t4_dp_hot_kernel( int n, int variant, const int *tw, const i64 *
 			d.alCap = small ? (int)sizeof( wal[0] ) : 2 * d.n + 8 ;
 			d.al = small ? wal[h] : (signed char *)( scratch + scratchOff[k] + 13 * d.actStride ) ;
 		}
+		__syncwarp() ;
 		T4SideStats r[2] ;
 		w_side_pair( cx, s[0], s[1], nib, bits, r[0], r[1] ) ;
 		for ( int h = 0 ; h < 2 ; ++h )
@@ -231,7 +235,10 @@ __global__ void t4_dp_hot_kernel( int n, int variant, const int *tw, const i64 *
 	T4Ctx cx ;
 	cx.tid = lane ;
 	cx.nt = 32 ;
-	int matches = w_stage_side( t, pp, len, nib[0], bits[0], lane ) ;
+	for ( int x = lane ; x < len ; x += 32 )
+		eqb[0][x] = (unsigned char)t4_eq_nibble( t + 4 * x ) ;
+	__syncwarp() ;
+	int matches = w_stage_side( eqb[0], pp, len, nib[0], bits[0], lane ) ;
 	(void)matches ;
 	const bool small = len < 16 * T4_WACT_WORDS ;
 	const int actStride = small ? T4_WACT_WORDS : ( len / 16 + 2 ) ;
@@ -1301,6 +1308,35 @@ int64_t T4_API( seqset_index_checksum )( t4_seqset *s, uint64_t *checksum )
 	}
 	*checksum = sum ;
 	return total ;
+}
+
+// Every live column's equality byte against its posWeight counts (test hook of the t4_eq cache)
+int64_t T4_API( test_check_eq_bytes )( t4_seqset *s, int64_t *bad )
+{
+	T4Stream st ;
+	int r = get_stream( s, &st ) ;
+	if ( r ) return r ;
+	std::vector<T4Contig> ct( st.nSeqs ) ;
+	if ( st.nSeqs && ( r = d2h( ct.data(), E.A + st.seqsOff, (size_t)st.nSeqs * sizeof( T4Contig ) ) ) )
+		return r ;
+	int64_t cols = 0, nbad = 0 ;
+	std::vector<int32_t> pw ;
+	std::vector<unsigned char> eq ;
+	for ( const T4Contig &k : ct )
+	{
+		if ( !k.consOff )
+			continue ;
+		pw.resize( 4 * (size_t)k.len ) ;
+		eq.resize( k.len ) ;
+		if ( ( r = d2h( pw.data(), E.A + k.pwOff + 16ull * k.lead, 16ull * k.len ) )
+			|| ( r = d2h( eq.data(), E.A + k.pwOff + 16ull * k.cap + k.lead, k.len ) ) )
+			return r ;
+		for ( int i = 0 ; i < k.len ; ++i )
+			nbad += eq[i] != t4_eq_nibble( pw.data() + 4 * i ) ;
+		cols += k.len ;
+	}
+	*bad = nbad ;
+	return cols ;
 }
 
 // ---- host utilities -----------------------------------------------------------

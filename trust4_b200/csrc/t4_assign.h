@@ -93,9 +93,14 @@ T4_D inline void c_input_seqset( T4Ctx &cx, const T4Stream *src )
 		int *pw = t4_pw( cx, c ) ;
 		const char *scons = cx.P<char>( sc->consOff ) + sc->lead ;
 		const int *spw = cx.P<int>( sc->pwOff ) + 4 * sc->lead ;
+		unsigned char *eq = t4_eq( cx, c ) ;
+		const unsigned char *seqb = cx.P<unsigned char>( sc->pwOff + 16ull * sc->cap ) + sc->lead ;
 		const int len = sc->len ;
 		T4_PAR_FOR( i, len )
+		{
 			cons[i] = scons[i] ;
+			eq[i] = seqb[i] ;
+		}
 		T4_PAR_FOR( i, 4 * len )
 			pw[i] = spw[i] ;
 		T4_SYNC() ;
@@ -449,10 +454,17 @@ T4_D inline void c_assign_recompute( T4Ctx &cx, T4Op *op )
 		if ( c->consOff == 0 )
 			continue ;
 		int *pw = t4_pw( cx, c ) ;
+		unsigned char *eq = t4_eq( cx, c ) ;
 		const char *cons = t4_cons( cx, c ) ;
+		// the counts were zeroed and added with atomics above: every column's equality byte is refreshed here, once
+		// they are final
 		T4_PAR_FOR( i, c->len )
+		{
 			if ( cons[i] != 'N' && pw[4 * i] + pw[4 * i + 1] + pw[4 * i + 2] + pw[4 * i + 3] == 0 )
-				pw[4 * i + t4_nuc( cons[i] )] = 1 ;
+				t4_col_add( pw, eq, i, t4_nuc( cons[i] ), 1 ) ;
+			else
+				eq[i] = (unsigned char)t4_eq_nibble( pw + 4 * i ) ;
+		}
 	}
 	T4_SYNC() ;
 	if ( cx.tid == 0 )

@@ -77,7 +77,7 @@ struct T4Dir               // one k-mer directory slot (32 B = one HBM sector); 
 struct T4Contig            // SeqSet.hpp:19 `_seqWrapper`, novel contigs only (isRef is always false in the stage-1 seqSet)
 {
 	u64 consOff ;          // char[cap], the consensus occupies [lead, lead + len)
-	u64 pwOff ;            // int32[4] per base, same lead
+	u64 pwOff ;            // int32[4][cap] per base, same lead, then u8[cap] equality bytes (t4_eq), same lead
 	u64 nameOff ;
 	int nameLen ;
 	int len ;              // consensusLen; alive iff consOff != 0

@@ -235,6 +235,35 @@ T4_D inline void s_refill_slab( T4Ctx &cx )
 T4_D inline T4Contig *t4_seq( T4Ctx &cx, int idx ) { return cx.P<T4Contig>( cx.st->seqsOff ) + idx ; }
 T4_D inline char *t4_cons( T4Ctx &cx, T4Contig *c ) { return cx.P<char>( c->consOff ) + c->lead ; }
 T4_D inline int *t4_pw( T4Ctx &cx, T4Contig *c ) { return cx.P<int>( c->pwOff ) + 4 * c->lead ; }
+// Equality byte of every posWeight column, stored behind the posWeight array of the same allocation (so T4Contig stays
+// two sectors and no contig can have counts without bytes): bit b set iff AlignAlgo::IsBaseEqual( column, base b )
+// (AlignAlgo.hpp:49-55, an 'N' read base matches everything at the consumer).  The overhang masks, the gap scoring and
+// the overhang DPs read one byte per column instead of four counts.
+T4_D inline unsigned char *t4_eq( T4Ctx &cx, T4Contig *c ) { return cx.P<unsigned char>( c->pwOff + 16ull * c->cap ) + c->lead ; }
+#define T4_PW_BYTES( cap ) ( (u64)( cap ) * 17 )
+
+T4_HD inline unsigned t4_eq_nibble( const int *w )
+{
+	int sum = w[0] + w[1] + w[2] + w[3] ;
+	if ( sum == 0 )
+		return 0xFu ;
+	return ( sum < 3 * w[0] ? 1u : 0u ) | ( sum < 3 * w[1] ? 2u : 0u ) | ( sum < 3 * w[2] ? 4u : 0u ) | ( sum < 3 * w[3] ? 8u : 0u ) ;
+}
+
+// Every store of posWeight counts goes through these two (or copies a column together with its byte), so the equality
+// byte stays a function of the column.  Column col of pw / eq (both from the contig's lead).
+T4_HD inline void t4_col_put( int *pw, unsigned char *eq, int col, int a, int c, int g, int t )
+{
+	int *w = pw + 4 * col ;
+	w[0] = a ; w[1] = c ; w[2] = g ; w[3] = t ;
+	eq[col] = (unsigned char)t4_eq_nibble( w ) ;
+}
+T4_HD inline void t4_col_add( int *pw, unsigned char *eq, int col, int b, int d )
+{
+	int *w = pw + 4 * col ;
+	w[b] += d ;
+	eq[col] = (unsigned char)t4_eq_nibble( w ) ;
+}
 
 T4_D inline u64 t4_key_of( int strand, int idx, int a, int b, int bigRepeat )
 {
@@ -722,7 +751,7 @@ T4_D inline int s_new_contig( T4Ctx &cx, int len )
 	T4Contig *c = t4_seq( cx, idx ) ;
 	int cap = 2 * len + 128 ;
 	c->consOff = s_alloc( cx, cap ) ;
-	c->pwOff = s_alloc( cx, (u64)cap * 16 ) ;
+	c->pwOff = s_alloc( cx, T4_PW_BYTES( cap ) ) ;
 	if ( !c->consOff || !c->pwOff )
 		return -1 ;
 	c->cap = cap ;
@@ -757,18 +786,22 @@ T4_D inline bool s_contig_grow( T4Ctx &cx, T4Contig *c, int left, int right )
 	}
 	int cap = 2 * newLen + 128 ;
 	u64 co = s_alloc( cx, cap ) ;
-	u64 po = s_alloc( cx, (u64)cap * 16 ) ;
+	u64 po = s_alloc( cx, T4_PW_BYTES( cap ) ) ;
 	if ( !co || !po )
 		return false ;
 	int lead = ( cap - newLen ) / 2 ;
 	char *oc = t4_cons( cx, c ) ;
 	int *op = t4_pw( cx, c ) ;
+	const unsigned char *oe = t4_eq( cx, c ) ;
 	char *nc = cx.P<char>( co ) + lead + left ;
 	int *np = cx.P<int>( po ) + 4 * ( lead + left ) ;
+	unsigned char *ne = cx.P<unsigned char>( po + 16ull * cap ) + lead + left ;
 	for ( int i = 0 ; i < c->len ; ++i )
 		nc[i] = oc[i] ;
 	for ( int i = 0 ; i < 4 * c->len ; ++i )
 		np[i] = op[i] ;
+	for ( int i = 0 ; i < c->len ; ++i )
+		ne[i] = oe[i] ;
 	c->consOff = co ;
 	c->pwOff = po ;
 	c->cap = cap ;
@@ -1254,14 +1287,6 @@ T4_HD inline void t4_dp_one( const T4DpParams &P, i64 i )
 // Both score rows live in registers (the 13-wide window is fully unrolled), IsBaseEqual outcomes slide through a
 // 64-bit register as one nibble per column (bit b = "base b equals this column"), and the traceback decision of a
 // row is packed into one 32-bit word (2 bits per band cell).  act32: n + 1 words.
-T4_HD inline unsigned t4_eq_nibble( const int *w )
-{
-	int sum = w[0] + w[1] + w[2] + w[3] ;
-	if ( sum == 0 )
-		return 0xFu ;
-	return ( sum < 3 * w[0] ? 1u : 0u ) | ( sum < 3 * w[1] ? 2u : 0u ) | ( sum < 3 * w[2] ? 4u : 0u ) | ( sum < 3 * w[3] ? 8u : 0u ) ;
-}
-
 T4_HD inline int t4_dp_equal( const int *tw, const char *p, int n, signed char *align, u32 *act32, bool diagKnownBad, int *usedFullDp )
 {
 	if ( usedFullDp )
@@ -2465,11 +2490,10 @@ T4_D inline int w_dp_equal_half( T4Ctx &cx, const u32 *nib, const char *p, int n
 	return ret ;
 }
 
-// Stage one side for a warp: the n columns tw[0..n) against p[0..n): IsBaseEqual nibbles (8 per word) and the
-// match bits, into shared memory, with coalesced 16-byte column loads.  Returns the number of matches.
-T4_D inline int w_stage_side( const int *tw, const char *p, int n, u32 *nibOut, u32 *bitsOut, int lane )
+// Stage one side for a warp: the n columns with equality bytes te[0..n) (t4_eq) against p[0..n): IsBaseEqual
+// nibbles (8 per word) and the match bits, into shared memory.  Returns the number of matches.
+T4_D inline int w_stage_side( const unsigned char *te, const char *p, int n, u32 *nibOut, u32 *bitsOut, int lane )
 {
-	const int4 *tw4 = (const int4 *)tw ;
 	int matches = 0 ;
 	for ( int t0 = 0 ; t0 < n ; t0 += 32 )
 	{
@@ -2478,9 +2502,7 @@ T4_D inline int w_stage_side( const int *tw, const char *p, int n, u32 *nibOut, 
 		bool eq = false ;
 		if ( t < n )
 		{
-			int4 w = tw4[t] ;
-			int sum = w.x + w.y + w.z + w.w ;
-			nb = ( sum == 0 ) ? 0xFu : ( ( sum < 3 * w.x ? 1u : 0u ) | ( sum < 3 * w.y ? 2u : 0u ) | ( sum < 3 * w.z ? 4u : 0u ) | ( sum < 3 * w.w ? 8u : 0u ) ) ;
+			nb = te[t] ;
 			char pc = p[t] ;
 			eq = ( pc == 'N' ) || ( ( nb >> t4_nuc( pc ) ) & 1u ) ;
 		}
@@ -2534,11 +2556,11 @@ T4_D inline T4SideStats w_side_stats( const T4AlignView &v, bool fromEnd, int la
 	return r ;
 }
 
-// One overhang side of w_side_pair: n columns tw[0..n) against p[0..n) (n == 0: no side); fromEnd for a left
-// overhang.  act / actStride: the traceback words of its half-warp DP; al / alCap: its edit-string buffer.
+// One overhang side of w_side_pair: n columns with equality bytes te[0..n) against p[0..n) (n == 0: no side); fromEnd
+// for a left overhang.  act / actStride: the traceback words of its half-warp DP; al / alCap: its edit-string buffer.
 struct T4DpSide
 {
-	const int *tw ;
+	const unsigned char *te ;
 	const char *p ;
 	int n ;
 	bool fromEnd ;
@@ -2554,8 +2576,8 @@ T4_D inline void w_side_pair( T4Ctx &cx, const T4DpSide &s0, const T4DpSide &s1,
 	T4SideStats &r0, T4SideStats &r1 )
 {
 	const int lane = cx.tid & 31 ;
-	w_stage_side( s0.tw, s0.p, s0.n, nib[0], bits[0], lane ) ;
-	w_stage_side( s1.tw, s1.p, s1.n, nib[1], bits[1], lane ) ;
+	w_stage_side( s0.te, s0.p, s0.n, nib[0], bits[0], lane ) ;
+	w_stage_side( s1.te, s1.p, s1.n, nib[1], bits[1], lane ) ;
 	const bool hi = lane >= 16 ;
 	int alen = 0 ;
 	w_dp_equal_half( cx, nib[hi ? 1 : 0], hi ? s1.p : s0.p, hi ? s1.n : s0.n, hi ? s1.al : s0.al, hi ? s1.alCap : s0.alCap, &alen,
@@ -2593,7 +2615,7 @@ T4_D inline void c_score_all_warp( T4Ctx &cx, T4Ovl *ovl, int overlapCnt, const 
 		const char *r = ( o.strand == 1 ) ? sm->read : sm->rc ;
 		const u64 *hc = keys + o.hcStart ;
 		const int hitCnt = o.hcCnt ;
-		const int *pw = t4_pw( cx, t4_seq( cx, o.seqIdx ) ) ;
+		const unsigned char *eqb = t4_eq( cx, t4_seq( cx, o.seqIdx ) ) ;
 		int acc = 0 ;           // per-lane partial of matchCnt
 		bool fail = false ;
 		for ( int base = 1 ; base < hitCnt && !fail ; base += 32 )
@@ -2625,10 +2647,9 @@ T4_D inline void c_score_all_warp( T4Ctx &cx, T4Ovl *ovl, int overlapCnt, const 
 					fail = true ;
 					break ;
 				}
-				const int *tw = pw + 4 * ( gb0 + k ) ;
 				const char *p = r + ga0 + k ;
 				// IsBaseEqual along the diagonal of the gap (nibbles + match bits staged in shared memory)
-				int matches = w_stage_side( tw, p, gap, sm->wnib[warp][0], sm->wbits[warp][0], lane ) ;
+				int matches = w_stage_side( eqb + gb0 + k, p, gap, sm->wnib[warp][0], sm->wbits[warp][0], lane ) ;
 				int cnt0 = matches ;
 				if ( gap >= 2 && SCORE_MATCH * matches + SCORE_MISMATCH * ( gap - matches ) < gap * SCORE_MATCH + 2 * SCORE_INDEL )
 				{
@@ -3165,6 +3186,7 @@ T4_D inline int c_input_novel_read( T4Ctx &cx, const char *id, int idLen, int le
 	T4Contig *c = t4_seq( cx, seqIdx ) ;
 	char *cons = t4_cons( cx, c ) ;
 	int *pw = t4_pw( cx, c ) ;
+	unsigned char *eq = t4_eq( cx, c ) ;
 	const char *src = ( strand == -1 ) ? sm->rc : sm->read ;
 	T4_PAR_FOR( i, len )
 	{
@@ -3176,7 +3198,7 @@ T4_D inline int c_input_novel_read( T4Ctx &cx, const char *id, int idLen, int le
 			int x = t4_nuc( ch ) ;
 			w0 = x == 0 ; w1 = x == 1 ; w2 = x == 2 ; w3 = x == 3 ;
 		}
-		pw[4 * i] = w0 ; pw[4 * i + 1] = w1 ; pw[4 * i + 2] = w2 ; pw[4 * i + 3] = w3 ;
+		t4_col_put( pw, eq, i, w0, w1, w2, w3 ) ;
 	}
 	T4_SYNC() ;
 	c_index_op( cx, cons, len, T4_IDX_BUILD, seqIdx, barcode, 0, 0 ) ;
@@ -3195,11 +3217,12 @@ T4_D inline int c_repeat_add_read( T4Ctx &cx, int len )
 	const char *r = ( st->prevStrand == -1 ) ? cx.sm->rc : cx.sm->read ;
 	T4Contig *seq = t4_seq( cx, st->prevSeqIdx ) ;
 	int *pw = t4_pw( cx, seq ) ;
+	unsigned char *eq = t4_eq( cx, seq ) ;
 	for ( int i = st->prevReadStart + cx.tid ; i <= st->prevReadEnd ; i += cx.nt )
 	{
 		if ( r[i] == 'N' )
 			continue ;
-		++pw[4 * ( i + st->prevSeqStart ) + t4_nuc( r[i] )] ;
+		t4_col_add( pw, eq, i + st->prevSeqStart, t4_nuc( r[i] ), 1 ) ;
 	}
 	T4_SYNC() ;
 	if ( cx.tid == 0 )
@@ -3218,11 +3241,12 @@ T4_D inline int c_repeat_add_read_n( T4Ctx &cx, int len, int L )
 	const char *r = ( st->prevStrand == -1 ) ? cx.sm->rc : cx.sm->read ;
 	T4Contig *seq = t4_seq( cx, st->prevSeqIdx ) ;
 	int *pw = t4_pw( cx, seq ) ;
+	unsigned char *eq = t4_eq( cx, seq ) ;
 	for ( int i = st->prevReadStart + cx.tid ; i <= st->prevReadEnd ; i += cx.nt )
 	{
 		if ( r[i] == 'N' )
 			continue ;
-		pw[4 * ( i + st->prevSeqStart ) + t4_nuc( r[i] )] += L ;
+		t4_col_add( pw, eq, i + st->prevSeqStart, t4_nuc( r[i] ), L ) ;
 	}
 	T4_SYNC() ;
 	if ( cx.tid == 0 )
@@ -3282,19 +3306,21 @@ T4_D inline void s_make_exact( T4Ctx &cx, const char *r, int len, double factor,
 #endif
 }
 
-// Overhang side x = 2 i + right of overlap o = overlaps[i]: its posWeight columns *tw and read bases *p.  Returns its length.
-T4_D inline int t4_side_span( T4Ctx &cx, const T4Ovl &o, int right, const char *r, int len, const int **tw, const char **p )
+// Overhang side x = 2 i + right of overlap o = overlaps[i]: its posWeight columns *tw, their equality bytes *te and
+// read bases *p.  Returns its length.
+T4_D inline int t4_side_span( T4Ctx &cx, const T4Ovl &o, int right, const char *r, int len, const int **tw,
+	const unsigned char **te, const char **p )
 {
 	T4Contig *seq = t4_seq( cx, o.seqIdx ) ;
-	const int *pw = t4_pw( cx, seq ) ;
+	const int col = right ? o.seqEnd + 1 : o.seqStart - t4_min( o.readStart, o.seqStart ) ;
+	*tw = t4_pw( cx, seq ) + 4 * col ;
+	*te = t4_eq( cx, seq ) + col ;
 	if ( !right )
 	{
 		int L = t4_min( o.readStart, o.seqStart ) ;
-		*tw = pw + 4 * ( o.seqStart - L ) ;
 		*p = r + o.readStart - L ;
 		return L ;
 	}
-	*tw = pw + 4 * ( o.seqEnd + 1 ) ;
 	*p = r + o.readEnd + 1 ;
 	return t4_min( len - 1 - o.readEnd, seq->len - 1 - o.seqEnd ) ;
 }
@@ -3318,9 +3344,10 @@ T4_D inline void c_overhang_dps( T4Ctx &cx, const T4Ovl *overlaps, const char *r
 		{
 			T4DpSide &d = s[h] ;
 			const int x = ( q + h < cnt ) ? pend[q + h] : -1 ;
-			d.tw = 0 ;
+			const int *tw = 0 ;
+			d.te = 0 ;
 			d.p = 0 ;
-			d.n = ( x >= 0 ) ? t4_side_span( cx, overlaps[x >> 1], x & 1, r, len, &d.tw, &d.p ) : 0 ;
+			d.n = ( x >= 0 ) ? t4_side_span( cx, overlaps[x >> 1], x & 1, r, len, &tw, &d.te, &d.p ) : 0 ;
 			d.fromEnd = !( x & 1 ) ;
 			const bool small = d.n < 16 * T4_WACT_WORDS ;
 			d.act = small ? sm->wact[warp][h] : (u32 *)t4_dp_scratch_of( cx, warp * 32 + 16 * h ).act ;
@@ -3344,8 +3371,10 @@ T4_D inline void c_overhang_dps( T4Ctx &cx, const T4Ovl *overlaps, const char *r
 	{
 		const int x = pend[q] ;
 		const int *tw ;
+		const unsigned char *te ;
 		const char *p ;
-		const int n = t4_side_span( cx, overlaps[x >> 1], x & 1, r, len, &tw, &p ) ;
+		const int n = t4_side_span( cx, overlaps[x >> 1], x & 1, r, len, &tw, &te, &p ) ;
+		(void)te ;
 		T4AlignView av = t4_overhang_align( tw, p, n, bits + 32 * ( x >> 1 ) + 16 * ( x & 1 ), ds ) ;
 		if ( av.dp )
 			t4_count( cx, 1, 1 ) ;
@@ -3355,65 +3384,73 @@ T4_D inline void c_overhang_dps( T4Ctx &cx, const T4Ovl *overlaps, const char *r
 	T4_SYNC() ;
 }
 
-// IsBaseEqual( posWeight column, read base ) of every overhang column of every overlap (ExtendOverlap, SeqSet.hpp:1165-1175) as bit
+// IsBaseEqual( column, read base ) from the column's equality byte (t4_eq): an 'N' read base matches every column.
+T4_HD inline bool t4_eq_hit( unsigned b, char pc ) { return pc == 'N' || ( ( b >> t4_nuc( pc ) ) & 1u ) ; }
+
+// A side of n overhang columns with `matches` diagonal matches needs the banded DP (AlignAlgo.hpp:59-103: more than
+// 2 mismatches on the diagonal).
+T4_HD inline bool t4_side_needs_dp( int n, int matches )
+{
+	return n >= 2 && ( SCORE_MATCH * matches + SCORE_MISMATCH * ( n - matches ) < n * SCORE_MATCH + 2 * SCORE_INDEL ) ;
+}
+
+#if T4_CUDA
+// The overhang masks of overlap o for one warp (ExtendOverlap, SeqSet.hpp:1165-1175): bit t of word w of a side is
+// IsBaseEqual( column, read base ) of overhang position 32 w + t.  Lane w < 16 returns word w of the left side, lane
+// 16 + w word w of the right side (the layout of st->bitsOff), zero beyond the side; *nL / *nR get the side lengths.
+// The equality bytes of both sides are loaded 8 words at a time (one round trip for overhangs up to 256 columns)
+// before any of them is used.
+T4_D inline u32 w_overhang_masks( T4Ctx &cx, const T4Ovl &o, const char *r, int len, int lane, int *nL, int *nR )
+{
+	T4Contig *seq = t4_seq( cx, o.seqIdx ) ;
+	const unsigned char *eq = t4_eq( cx, seq ) ;
+	const int L = t4_min( o.readStart, o.seqStart ) ;
+	const int R = t4_min( len - 1 - o.readEnd, seq->len - 1 - o.seqEnd ) ;
+	const unsigned char *eL = eq + o.seqStart - L, *eR = eq + o.seqEnd + 1 ;
+	const char *pL = r + o.readStart - L, *pR = r + o.readEnd + 1 ;
+	const int nw = ( t4_max( L, R ) + 31 ) >> 5 ;
+	u32 mine = 0 ;
+	for ( int w0 = 0 ; w0 < nw ; w0 += 8 )
+	{
+		unsigned bl[8], br[8] ;
+#pragma unroll
+		for ( int u = 0 ; u < 8 ; ++u )
+		{
+			const int t = 32 * ( w0 + u ) + lane ;
+			bl[u] = t < L ? eL[t] : 0u ;
+			br[u] = t < R ? eR[t] : 0u ;
+		}
+#pragma unroll
+		for ( int u = 0 ; u < 8 ; ++u )
+		{
+			const int t = 32 * ( w0 + u ) + lane ;
+			const u32 ml = __ballot_sync( T4_FULL, t < L && t4_eq_hit( bl[u], pL[t] ) ) ;
+			const u32 mr = __ballot_sync( T4_FULL, t < R && t4_eq_hit( br[u], pR[t] ) ) ;
+			if ( lane == w0 + u )
+				mine = ml ;
+			if ( lane == 16 + w0 + u )
+				mine = mr ;
+		}
+	}
+	*nL = L ;
+	*nR = R ;
+	return mine ;
+}
+#endif
+
+// IsBaseEqual( column, read base ) of every overhang column of every overlap (ExtendOverlap, SeqSet.hpp:1165-1175) as bit
 // masks: bits[32 * i + 16 * side + w] holds overhang positions 32 w .. 32 w + 31 of side (0 left, 1 right) of overlap i.
 // Collective; r is the read in the strand of the overlaps.
 T4_D inline void c_overhang_bits( T4Ctx &cx, const T4Ovl *overlaps, int overlapCnt, const char *r, int len, u32 *bits )
 {
 #if T4_CUDA
+	const int warp = cx.tid >> 5, nwarps = cx.nt >> 5, lane = cx.tid & 31 ;
+	for ( int oi = warp ; oi < overlapCnt ; oi += nwarps )
 	{
-		// one warp per overlap (metadata fetched once), then per 32-column word lane t loads column t
-		// (one coalesced 512-byte request) and a ballot forms the word
-		const int warp = cx.tid >> 5, nwarps = cx.nt >> 5, lane = cx.tid & 31 ;
-		for ( int oi = warp ; oi < overlapCnt ; oi += nwarps )
-		{
-			const T4Ovl o = overlaps[oi] ;
-			T4Contig *seq = t4_seq( cx, o.seqIdx ) ;
-			const int seqLen = seq->len ;
-			const int4 *pw4 = (const int4 *)t4_pw( cx, seq ) ;
-			for ( int right = 0 ; right < 2 ; ++right )
-			{
-				int n, col0, rp0 ;
-				if ( !right )
-				{
-					n = t4_min( o.readStart, o.seqStart ) ;
-					col0 = o.seqStart - n ;
-					rp0 = o.readStart - n ;
-				}
-				else
-				{
-					n = t4_min( len - 1 - o.readEnd, seqLen - 1 - o.seqEnd ) ;
-					col0 = o.seqEnd + 1 ;
-					rp0 = o.readEnd + 1 ;
-				}
-				u32 *out = bits + 32 * oi + 16 * right ;
-				for ( int w = 0 ; w < 16 ; ++w )
-				{
-					if ( w * 32 >= n )
-					{
-						if ( lane == 0 )
-							out[w] = 0 ;
-						continue ;
-					}
-					int t = w * 32 + lane ;
-					bool eq = false ;
-					if ( t < n )
-					{
-						const int4 wv = pw4[col0 + t] ;
-						char pc = r[rp0 + t] ;
-						int c = t4_nuc( pc ) ;
-						int sum = wv.x + wv.y + wv.z + wv.w ;
-						int wc = c == 0 ? wv.x : ( c == 1 ? wv.y : ( c == 2 ? wv.z : wv.w ) ) ;
-						eq = ( sum == 0 || pc == 'N' || sum < 3 * wc ) ;
-					}
-					unsigned m = __ballot_sync( 0xffffffffu, eq ) ;
-					if ( lane == 0 )
-						out[w] = m ;
-				}
-			}
-		}
+		const T4Ovl o = overlaps[oi] ;
+		int nL, nR ;
+		bits[32 * oi + lane] = w_overhang_masks( cx, o, r, len, lane, &nL, &nR ) ;
 	}
-	T4_SYNC() ;
 #else
 	T4_PAR_FOR( x, overlapCnt * 32 )
 	{
@@ -3436,16 +3473,132 @@ T4_D inline void c_overhang_bits( T4Ctx &cx, const T4Ovl *overlaps, int overlapC
 		u32 m = 0 ;
 		if ( w * 32 < n )
 		{
-			const int *pw = t4_pw( cx, seq ) ;
+			const unsigned char *eq = t4_eq( cx, seq ) ;
 			int hi = n - w * 32 < 32 ? n - w * 32 : 32 ;
 			for ( int t = 0 ; t < hi ; ++t )
-				if ( t4_base_equal( pw + 4 * ( col0 + w * 32 + t ), r[rp0 + w * 32 + t] ) )
+				if ( t4_eq_hit( eq[col0 + w * 32 + t], r[rp0 + w * 32 + t] ) )
 					m |= 1u << t ;
 		}
 		bits[x] = m ;
 	}
-	T4_SYNC() ;
 #endif
+	T4_SYNC() ;
+}
+
+// Lazy ExtendOverlap: pre[i] of c_add_read from the statistics of overlap i's two sides (ind == -1: deferred to the
+// banded DP).  With both sides settled it is the exact result (state 2: hcCnt 2, infoFromHits = the return value).
+// Otherwise, when the return value alone matters (the bridging loop, SeqSet.hpp:3736-3750), an overlap is skipped
+// without any DP if ExtendOverlap provably returns 0 (state 1): with the total diagonal mismatch count M over the
+// mismatch budget and density, either every deferred side aligns without indel (then its counts ARE the diagonal
+// counts and the budget test fails) or some side has an indel (ret = 0).  State 0 leaves it to the DP pass.
+T4_D inline T4Ovl t4_settle_overlap( T4Ctx &cx, int len, T4Contig *seq, double factor, const T4Ovl &o, const T4SideStats &ls,
+	const T4SideStats &rs )
+{
+	T4Ovl e = o ;
+	if ( ls.ind == 0 && rs.ind == 0 )
+	{
+		int ok = t4_extend_finish( cx, len, seq, factor, o, e, ls, rs ) ;
+		e.infoFromHits = ok ; // aux: the return value
+		e.hcCnt = 2 ;         // aux: exact
+	}
+	else
+	{
+		int L = t4_min( o.readStart, o.seqStart ) ;
+		int R = t4_min( len - 1 - o.readEnd, seq->len - 1 - o.seqEnd ) ;
+		int M = ls.x + rs.x ;
+		int thr = 2 + ( L >= 2 ? 1 : 0 ) + ( R >= 2 ? 1 : 0 ) ;
+		thr = (int)( thr * factor ) ;
+		bool surely0 = ( M > thr ) && ( (double)M / ( L + R ) > 1.5 / cx.st->kmerLength ) ;
+		e.infoFromHits = 0 ;
+		e.hcCnt = surely0 ? 1 : 0 ;
+	}
+	return e ;
+}
+
+// ExtendOverlap's overhang masks and side statistics of every overlap, and pre[i] (t4_settle_overlap); the sides that
+// need the DP get ind == -1 in sstats[2 i + side].  The masks also go to bits (the DPs of the emulation and
+// s_make_exact read them).  Collective.  On the device one warp takes an overlap at a time: record and contig header
+// once, the equality bytes of both sides in one batch, the masks in registers (and the warp's shared words for the
+// statistics), then lane 0 settles the overlap -- no CTA barrier between masks and results.
+T4_D inline void c_overhang_settle( T4Ctx &cx, const T4Ovl *overlaps, int overlapCnt, const char *r, int len, double factor,
+	u32 *bits, T4SideStats *sstats, T4Ovl *pre )
+{
+#if T4_CUDA
+	const int warp = cx.tid >> 5, nwarps = cx.nt >> 5, lane = cx.tid & 31 ;
+	u32 *wb = &cx.sm->wbits[warp][0][0] ; // [side][word], the layout of one overlap's 32 words of bits
+	for ( int oi = warp ; oi < overlapCnt ; oi += nwarps )
+	{
+		const T4Ovl o = overlaps[oi] ;
+		int n[2] ;
+		const u32 mine = w_overhang_masks( cx, o, r, len, lane, &n[0], &n[1] ) ;
+		bits[32 * oi + lane] = mine ;
+		wb[lane] = mine ;
+		int mc = __popc( mine ) ;
+		mc += __shfl_xor_sync( T4_FULL, mc, 8 ) ;
+		mc += __shfl_xor_sync( T4_FULL, mc, 4 ) ;
+		mc += __shfl_xor_sync( T4_FULL, mc, 2 ) ;
+		mc += __shfl_xor_sync( T4_FULL, mc, 1 ) ;
+		const int matches[2] = { __shfl_sync( T4_FULL, mc, 0 ), __shfl_sync( T4_FULL, mc, 16 ) } ;
+		__syncwarp() ;
+		T4SideStats ss[2] ;
+#pragma unroll
+		for ( int right = 0 ; right < 2 ; ++right )
+		{
+			if ( !t4_side_needs_dp( n[right], matches[right] ) )
+			{
+				T4AlignView av ;
+				av.a = 0 ; av.bits = wb + 16 * right ; av.n = n[right] ; av.dp = 0 ;
+				ss[right] = w_side_stats( av, !right, lane ) ;
+			}
+			else
+			{
+				ss[right].m = matches[right] ;
+				ss[right].x = n[right] - matches[right] ;
+				ss[right].ind = -1 ; // deferred
+				ss[right].good = 0 ;
+			}
+		}
+		if ( lane == 0 )
+		{
+			sstats[2 * oi] = ss[0] ;
+			sstats[2 * oi + 1] = ss[1] ;
+			pre[oi] = t4_settle_overlap( cx, len, t4_seq( cx, o.seqIdx ), factor, o, ss[0], ss[1] ) ;
+		}
+		__syncwarp() ;
+	}
+#else
+	c_overhang_bits( cx, overlaps, overlapCnt, r, len, bits ) ;
+	T4_PAR_FOR( i, overlapCnt )
+	{
+		const T4Ovl &o = overlaps[i] ;
+		T4Contig *seq = t4_seq( cx, o.seqIdx ) ;
+		T4SideStats ss[2] ;
+		for ( int right = 0 ; right < 2 ; ++right )
+		{
+			int n = right ? t4_min( len - 1 - o.readEnd, seq->len - 1 - o.seqEnd ) : t4_min( o.readStart, o.seqStart ) ;
+			const u32 *bb = bits + 32 * i + 16 * right ;
+			int matches = 0 ;
+			for ( int w = 0 ; w * 32 < n ; ++w )
+				matches += __builtin_popcount( bb[w] ) ;
+			if ( !t4_side_needs_dp( n, matches ) )
+			{
+				T4AlignView av ;
+				av.a = 0 ; av.bits = bb ; av.n = n ; av.dp = 0 ;
+				ss[right] = t4_side_stats( av, !right ) ;
+			}
+			else
+			{
+				ss[right].m = matches ;
+				ss[right].x = n - matches ;
+				ss[right].ind = -1 ; // deferred
+				ss[right].good = 0 ;
+			}
+			sstats[2 * i + right] = ss[right] ;
+		}
+		pre[i] = t4_settle_overlap( cx, len, seq, factor, o, ss[0], ss[1] ) ;
+	}
+#endif
+	T4_SYNC() ;
 }
 
 // ---------------------------------------------------------------------------
@@ -3508,93 +3661,21 @@ T4_D T4_BIG int c_add_read( T4Ctx &cx, int len, const char *geneName, int &stran
 	T4Ovl *pre = cx.P<T4Ovl>( st->extOff ) ;
 	{
 		{
-		// IsBaseEqual of every overhang column, 32 positions per work item, spread over the CTA
+		// masks, side statistics and pre[] of every overlap; the DP sides are deferred to c_overhang_dps below, which may
+		// leave an overlap to the decision loop to make exact on demand (s_make_exact)
 #if T4_CUDA
 		long long xt0 = clock64() ;
 #endif
 		u32 *bits = cx.P<u32>( st->bitsOff ) ;
-		c_overhang_bits( cx, overlaps, overlapCnt, r, len, bits ) ;
+		T4SideStats *sstats = (T4SideStats *)cx.P<char>( st->failOff ) ; // scratch: 2 per overlap (failOff is unused until the decision)
+		c_overhang_settle( cx, overlaps, overlapCnt, r, len, factor, bits, sstats, pre ) ;
 #if T4_CUDA
 		long long xt1 = clock64() ;
 #endif
-		// Lazy ExtendOverlap.  One thread per (overlap, side) settles the sides that need no DP (<= 1 column, or <= 2
-		// mismatches on the diagonal, AlignAlgo.hpp:59-103) from the bit masks.  An overlap whose sides are all settled gets
-		// its exact result now (state 2).  Otherwise its DP sides are deferred to the pass below (c_overhang_dps), which
-		// may leave an overlap to the decision loop to make exact on demand (s_make_exact); when the return value alone matters (the bridging loop,
-		// SeqSet.hpp:3736-3750) an overlap is skipped without any DP if ExtendOverlap provably returns 0 (state 1): with the
-		// total diagonal mismatch count M over the mismatch budget and density, either every deferred side aligns without
-		// indel (then its counts ARE the diagonal counts and the budget test fails) or some side has an indel (ret = 0).
-		T4SideStats *sstats = (T4SideStats *)cx.P<char>( st->failOff ) ; // scratch: 2 per overlap (failOff is unused until the decision)
-		T4_PAR_FOR( x, 2 * overlapCnt )
-		{
-			int i = x >> 1, right = x & 1 ;
-			const T4Ovl &o = overlaps[i] ;
-			T4Contig *seq = t4_seq( cx, o.seqIdx ) ;
-			int n = right ? t4_min( len - 1 - o.readEnd, seq->len - 1 - o.seqEnd ) : t4_min( o.readStart, o.seqStart ) ;
-			const u32 *bb = bits + 32 * i + ( right ? 16 : 0 ) ;
-			int matches = 0 ;
-			for ( int w = 0 ; w * 32 < n ; ++w )
-			{
-				u32 v = bb[w] ;
-				if ( ( w + 1 ) * 32 > n )
-					v &= ( 1u << ( n - w * 32 ) ) - 1u ;
-#if T4_CUDA
-				matches += __popc( v ) ;
-#else
-				matches += __builtin_popcount( v ) ;
-#endif
-			}
-			T4SideStats ss ;
-			bool needDp = n >= 2 && ( SCORE_MATCH * matches + SCORE_MISMATCH * ( n - matches ) < n * SCORE_MATCH + 2 * SCORE_INDEL ) ;
-			if ( !needDp )
-			{
-				T4AlignView av ;
-				av.a = 0 ; av.bits = bb ; av.n = n ; av.dp = 0 ;
-				ss = t4_side_stats( av, !right ) ;
-				ss.ind = 0 ;
-			}
-			else
-			{
-				ss.m = matches ;
-				ss.x = n - matches ;
-				ss.ind = -1 ; // deferred
-				ss.good = 0 ;
-			}
-			sstats[x] = ss ;
-		}
-		T4_SYNC() ;
-		T4_PAR_FOR( i, overlapCnt )
-		{
-			const T4SideStats ls = sstats[2 * i], rs = sstats[2 * i + 1] ;
-			T4Ovl e = overlaps[i] ;
-			T4Contig *seq = t4_seq( cx, overlaps[i].seqIdx ) ;
-			if ( ls.ind == 0 && rs.ind == 0 )
-			{
-				int ok = t4_extend_finish( cx, len, seq, factor, overlaps[i], e, ls, rs ) ;
-				e.infoFromHits = ok ; // aux: the return value
-				e.hcCnt = 2 ;         // aux: exact
-			}
-			else
-			{
-				int L = t4_min( overlaps[i].readStart, overlaps[i].seqStart ) ;
-				int R = t4_min( len - 1 - overlaps[i].readEnd, seq->len - 1 - overlaps[i].seqEnd ) ;
-				int M = ls.x + rs.x ;
-				int thr = 2 + ( L >= 2 ? 1 : 0 ) + ( R >= 2 ? 1 : 0 ) ;
-				thr = (int)( thr * factor ) ;
-				bool surely0 = ( M > thr ) && ( (double)M / ( L + R ) > 1.5 / st->kmerLength ) ;
-				e.infoFromHits = 0 ;
-				e.hcCnt = surely0 ? 1 : 0 ;
-			}
-			pre[i] = e ;
-		}
-		T4_SYNC() ;
 		// Every deferred side the decision loop may consult is aligned now, in one parallel pass, except the sides of a
 		// provably-0 overlap of an easy read (the best overlap is settled, extends, clears the threshold and covers the
 		// whole read).  The decision loop then consults the other overlaps (almost) only through the bridging loop,
 		// where state 1 suffices; the rare overlap it consults without a result is made exact on demand (s_make_exact).
-#if T4_CUDA
-		long long xt2 = clock64() ;
-#endif
 		bool easy = ( pre[0].hcCnt == 2 && pre[0].infoFromHits == 1 && pre[0].similarity >= similarityThreshold
 			&& pre[0].readStart == 0 && pre[0].readEnd == len - 1 ) ;
 		int *pend = (int *)( sstats + 2 * overlapCnt ) ; // the sides to align, in side order (failOff holds a T4Ovl per overlap)
@@ -3624,6 +3705,9 @@ T4_D T4_BIG int c_add_read( T4Ctx &cx, int len, const char *geneName, int &stran
 		}
 #endif
 		T4_SYNC() ;
+#if T4_CUDA
+		long long xt2 = clock64() ;
+#endif
 		c_overhang_dps( cx, overlaps, r, len, bits, pend, sm->bi[0], sstats ) ;
 		T4_PAR_FOR( i, overlapCnt )
 		{
@@ -3962,11 +4046,12 @@ T4_D T4_BIG int c_add_read( T4Ctx &cx, int len, const char *geneName, int &stran
 					int oldLen = ns->len ;
 					int cap = 2 * newConsensusLen + 128 ;
 					u64 co = s_alloc( cx, cap ) ;
-					u64 po = s_alloc( cx, (u64)cap * 16 ) ;
+					u64 po = s_alloc( cx, T4_PW_BYTES( cap ) ) ;
 					if ( co && po )
 					{
 						int lead = ( cap - newConsensusLen ) / 2 ;
 						int *npw = cx.P<int>( po ) + 4 * lead ;
+						unsigned char *neq = cx.P<unsigned char>( po + 16ull * cap ) + lead ;
 						int *opw = t4_pw( cx, ns ) ;
 						for ( i = 0 ; i < 4 * newConsensusLen ; ++i )
 							npw[i] = 0 ;
@@ -3983,6 +4068,8 @@ T4_D T4_BIG int c_add_read( T4Ctx &cx, int len, const char *geneName, int &stran
 							for ( j = 0 ; j < 4 * c->len ; ++j )
 								npw[4 * seqOffset[i] + j] += cpw[j] ;
 						}
+						for ( i = 0 ; i < newConsensusLen ; ++i )
+							neq[i] = (unsigned char)t4_eq_nibble( npw + 4 * i ) ;
 						// name (SeqSet.hpp:4066-4096)
 						int nameIdx ;
 						for ( nameIdx = 0 ; nameIdx < eOverlapCnt ; ++nameIdx )
@@ -4129,15 +4216,16 @@ T4_D T4_BIG int c_add_read( T4Ctx &cx, int len, const char *geneName, int &stran
 			{
 				char *newConsensus = t4_cons( cx, seq ) ;
 				int *pw = t4_pw( cx, seq ) ;
+				unsigned char *eq = t4_eq( cx, seq ) ;
 				const int newConsensusLen = seq->len ;
 				T4_PAR_FOR( i, shift )
 					newConsensus[i] = r[i] ;
 				T4_PAR_FOR( x, rightAdd )
 					newConsensus[shift + oldLen + x] = r[e0.readEnd + 1 + x] ;
-				T4_PAR_FOR( i, 4 * shift )
-					pw[i] = 0 ;
-				T4_PAR_FOR( i, 4 * rightAdd )
-					pw[4 * ( shift + oldLen ) + i] = 0 ;
+				T4_PAR_FOR( i, shift )
+					t4_col_put( pw, eq, i, 0, 0, 0, 0 ) ;
+				T4_PAR_FOR( i, rightAdd )
+					t4_col_put( pw, eq, shift + oldLen + i, 0, 0, 0, 0 ) ;
 				T4_SYNC() ;
 				if ( e0.readEnd < len - 1 )
 				{
@@ -4169,7 +4257,7 @@ T4_D T4_BIG int c_add_read( T4Ctx &cx, int len, const char *geneName, int &stran
 							}
 							for ( int j = 0 ; j < 4 ; ++j )
 								if ( r[i + shift] != t4_numToNuc( j ) && pw[4 * ( i + shift ) + j] > 1 )
-									--pw[4 * ( i + shift ) + j] ;
+									t4_col_add( pw, eq, i + shift, j, -1 ) ;
 						}
 					}
 					if ( e0.readEnd < len - 1 && ( barcode == -1 || minKmerCount > 1 ) )
@@ -4194,7 +4282,7 @@ T4_D T4_BIG int c_add_read( T4Ctx &cx, int len, const char *geneName, int &stran
 							}
 							for ( int j = 0 ; j < 4 ; ++j )
 								if ( r[pos] != t4_numToNuc( j ) && pw[4 * seqPos + j] > 1 )
-									--pw[4 * seqPos + j] ;
+									t4_col_add( pw, eq, seqPos, j, -1 ) ;
 						}
 					}
 					if ( shift > 0 )
@@ -4230,6 +4318,7 @@ T4_D T4_BIG int c_add_read( T4Ctx &cx, int len, const char *geneName, int &stran
 		T4Contig *seq = t4_seq( cx, seqIdx ) ;
 		char *cons = t4_cons( cx, seq ) ;
 		int *pw = t4_pw( cx, seq ) ;
+		unsigned char *eq = t4_eq( cx, seq ) ;
 		if ( cx.tid == 0 )
 			sm->bi[0] = 0 ;
 		T4_SYNC() ;
@@ -4237,7 +4326,7 @@ T4_D T4_BIG int c_add_read( T4Ctx &cx, int len, const char *geneName, int &stran
 		{
 			if ( r[i] == 'N' )
 				continue ;
-			++pw[4 * ( i + readInConsensusOffset ) + t4_nuc( r[i] )] ;
+			t4_col_add( pw, eq, i + readInConsensusOffset, t4_nuc( r[i] ), 1 ) ;
 			if ( cons[i + readInConsensusOffset] == 'N' )
 				sm->bi[0] = 1 ;
 		}

@@ -75,10 +75,12 @@ T4_D inline void c_ref_input( T4Ctx &cx, T4Op *op )
 		T4Contig *c = t4_seq( cx, idx ) ;
 		char *cons = t4_cons( cx, c ) ;
 		int *pw = t4_pw( cx, c ) ;
+		unsigned char *eq = t4_eq( cx, c ) ;
 		T4_PAR_FOR( i, len )
+		{
 			cons[i] = src[i] ;
-		T4_PAR_FOR( i, 4 * len )
-			pw[i] = 0 ;
+			t4_col_put( pw, eq, i, 0, 0, 0, 0 ) ;
+		}
 		T4_SYNC() ;
 		c_index_op( cx, cons, len, T4_IDX_BUILD, idx, -1, 0, 0 ) ;
 	}
