@@ -136,15 +136,10 @@ T4_D inline void t4_count( T4Ctx &cx, int idx, u64 v )
 // ---------------------------------------------------------------------------
 T4_HD inline int t4_nuc( char c ) // nucToNum[c - 'A'] & 3 (main.cpp:39-42): A0 C1 G2 T3, N -> 0, anything else -> 3
 {
-	switch ( c )
-	{
-		case 'A': return 0 ;
-		case 'C': return 1 ;
-		case 'G': return 2 ;
-		case 'T': return 3 ;
-		case 'N': return 0 ;
-		default: return 3 ;
-	}
+	// two bits per letter 'A' .. 'Z' in one constant: as a switch this is a jump table, and the lanes of a warp, which
+	// hold different bases, take its branches one after the other
+	const unsigned d = (unsigned)(unsigned char)c - 'A' ;
+	return d < 26u ? (int)( ( 0xffffff3ffefdcull >> ( 2 * d ) ) & 3u ) : 3 ;
 }
 T4_HD inline char t4_numToNuc( int x ) { return "ACGT"[x & 3] ; }
 
