@@ -574,7 +574,7 @@ public:
 
 	// T4_BATCH_SORT() (opt-in, T4_SORT=1) in front of `std::sort( sortedReads.begin(), sortedReads.end() ) ;` (main.cpp:1078),
 	// which becomes the fall-back statement: the device returns the permutation of _sortRead::operator< (t4_sort_reads) and
-	// the records are moved accordingly.  Emulation-verified only so far.
+	// the records are moved accordingly.  Verified in whole runs through the emulation and on an H100 (tests/test_gpu_dropin.py).
 	template <class Reads>
 	bool BatchSort( Reads &sortedReads )
 	{
@@ -684,8 +684,8 @@ public:
 
 	// T4_BATCH_ANNOTATE() is the third inserted line of the batch route: `if ( !seqSet.BatchAnnotate( ... ) )` in front of the
 	// rough annotation loop (main.cpp:1084: `if ( threadCnt <= 1 ) { ... AnnotateRead( read, 0, ... ) ... } else { pthreads }`),
-	// which becomes the fall-back branch.  OPT-IN (T4_ANNOTATE=1): the device pass behind it (t4_refset_annotate) has been
-	// verified through the CPU emulation only so far.  The gene set is rebuilt on the device from the driver's -f file with
+	// which becomes the fall-back branch.  OPT-IN (T4_ANNOTATE=1); whole runs with it are verified through the CPU emulation
+	// and on an H100 (tests/test_gpu_dropin.py).  The gene set is rebuilt on the device from the driver's -f file with
 	// refSet's k, hitLenRequired and radius (main.cpp:766-771, 1082-1083); sortedReads[i].geneOverlap[0..3] receive what
 	// AnnotateRead would have stored (an entry without a gene: seqIdx -1, strand 1).
 	template <class Reads, class RefSet>

@@ -3,9 +3,11 @@ repository's C-ABI library must write the same _raw.out, _final.out and _assembl
 (oracle/_ref/trust4) -- flags, file formats and `run-trust4 --stage 1` compatibility included (SURVEY.md 8b).
 
 CPU variant: the binding linked against the test emulation of the engine (tests/emu).  GPU variant: the binding linked
-against libtrust4_b200.so.  Both are built here, at test time, by integration/Makefile into integration/_build/ (make
-rebuilds them whenever the adapter changes; the libraries are linked dynamically, so the current build is what runs).
-Compiling them needs the reference sources (main.cpp): where those are missing every test here skips with that reason.
+against libtrust4_b200.so.  Where the reference sources (main.cpp) are present, both are built here, at test time, by
+integration/Makefile into integration/_build/ (make rebuilds them whenever the adapter changes; the libraries are linked
+dynamically, so the current build is what runs).  Elsewhere the GPU variants are the ones the oracle build linked into
+oracle/_ref/ (oracle/Makefile); the emulation variants, which link tests/emu/libt4emu.so, skip there.
+Every GPU run sets T4_ARENA_MB (GPU_ARENA_MB, below).  More GPU runs of the drop-ins: test_gpu_dropin.py.
 Inputs are synthetic FASTQ generated here, or the reference's shipped example stored under tests/golden/."""
 import gzip
 import os
@@ -61,15 +63,48 @@ def write_barcode_inputs(tmp, nreads=1500, nclones=24, n_barcodes=6, seed=23):
     return ["-f", fa, "-u", os.path.join(tmp, "reads.fq"), "--barcode", os.path.join(tmp, "bc.fa")]
 
 
+# Device arena of a GPU drop-in run (t4_init reads T4_ARENA_MB; unset, it takes half of the free HBM, too much on a
+# shared card).  The bump arena is never reset during a run, so it holds every set the run creates: a stream shell is
+# 1.17 MB (t4_stream_footprint at 128 threads: mostly the per-thread DP scratch and the hit buffers); the rough annotation
+# and the AssignRead pass each add one shell per resident worker (132 SMs x 4 = 528 on an H100, 618 MB each), plus the
+# gene set, the S assembly sets and the S extended sets with their contigs, k-mer directories and postings (tens of MB
+# for the largest input here).  About 1.4 GB at S = 64; 4 GB leaves room for growth.  The rough annotation's 14 MB
+# per-worker work blocks (t4_annot_scratch_bytes for 65 536 hits: 7.4 GB over 528 workers) are cudaMalloc'ed outside
+# the arena and freed when the pass returns.
+GPU_ARENA_MB = 4096
+
+
+def dropin_env(binary, env=None):
+    """The environment of a drop-in run: `env` on top of the caller's, plus T4_ARENA_MB for the GPU binaries."""
+    e = dict(os.environ, **(env or {}))
+    if os.path.basename(binary).startswith("trust4_gpu"):
+        e.setdefault("T4_ARENA_MB", str(GPU_ARENA_MB))
+    return e
+
+
 def run_and_compare(binary, args, tmp, extra=(), env=None):
-    for exe, tag in ((STOCK, "stock"), (binary, "dropin")):
-        e = dict(os.environ, **env) if (env and exe is binary) else None
-        subprocess.run([exe, "-t", "1", "-o", os.path.join(tmp, tag)] + list(extra) + args, check=True,
-                       stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL, timeout=900, env=e)
+    """Runs the stock binary and `binary` on the same input at -t 1 and asserts that the three output files are
+    byte-identical; returns the drop-in's stderr."""
+    subprocess.run([STOCK, "-t", "1", "-o", os.path.join(tmp, "stock")] + list(extra) + args, check=True,
+                   stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL, timeout=900)
+    r = subprocess.run([binary, "-t", "1", "-o", os.path.join(tmp, "dropin")] + list(extra) + args, check=True,
+                       stdout=subprocess.DEVNULL, stderr=subprocess.PIPE, timeout=900, env=dropin_env(binary, env), text=True)
     for suf in SUFFIXES:
         a = open(os.path.join(tmp, "stock" + suf), "rb").read()
         b = open(os.path.join(tmp, "dropin" + suf), "rb").read()
-        assert len(a) > 0 and a == b, suf
+        # compared outside the assert: pytest's diff of two multi-megabyte byte strings would take minutes
+        same = a == b
+        assert len(a) > 0 and same, "%s differs from the stock binary's: %s" % (suf, first_difference(a, b))
+    return r.stderr
+
+
+def first_difference(a, b):
+    """Where two outputs part: line number and both lines."""
+    la, lb = a.split(b"\n"), b.split(b"\n")
+    for i, (x, y) in enumerate(zip(la, lb)):
+        if x != y:
+            return "line %d: %r vs %r" % (i + 1, x[:200], y[:200])
+    return "%d vs %d lines" % (len(la), len(lb))
 
 
 def example_inputs(tmp):
@@ -82,13 +117,18 @@ def example_inputs(tmp):
 
 
 def dropin_binary(name):
-    """integration/_build/<name>, (re)built by integration/Makefile; skips where the reference sources are missing."""
-    if subprocess.run(["make", "-s", "-C", INTEGRATION, "has-reference"], stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL).returncode:
-        pytest.skip("reference sources not present (the drop-in binaries compile its main.cpp)")
+    """integration/_build/<name>, (re)built by integration/Makefile where the reference sources are present, so that a
+    test never runs a binary older than the adapter.  Elsewhere the GPU binaries that the oracle build linked
+    (oracle/_ref/trust4_gpu, trust4_gpu_batch); skips when neither exists."""
     if not os.path.exists(STOCK):
         pytest.skip("oracle/_ref/trust4 not built")
-    subprocess.run(["make", "-C", INTEGRATION, "_build/" + name], check=True, stdout=subprocess.DEVNULL)
-    return os.path.join(INTEGRATION, "_build", name)
+    if subprocess.run(["make", "-s", "-C", INTEGRATION, "has-reference"], stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL).returncode == 0:
+        subprocess.run(["make", "-C", INTEGRATION, "_build/" + name], check=True, stdout=subprocess.DEVNULL)
+        return os.path.join(INTEGRATION, "_build", name)
+    built = os.path.join(ROOT, "oracle", "_ref", name)
+    if os.path.exists(built):
+        return built
+    pytest.skip("reference sources not present (the drop-in binaries compile its main.cpp) and oracle/_ref/%s not built" % name)
 
 
 @pytest.fixture(scope="module")

@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 
 import barcode_cases as bcc
-from test_dropin_cli import STOCK, SUFFIXES, dropin_binary, write_barcode_inputs
+from test_dropin_cli import STOCK, SUFFIXES, dropin_binary, dropin_env, write_barcode_inputs
 
 
 @pytest.mark.parametrize("case", sorted(bcc.STATS_CASES))
@@ -42,7 +42,7 @@ def run_barcode_dropin(binary, tmp, extra):
     args = write_barcode_inputs(tmp)
     subprocess.run([STOCK, "-t", "1", "-o", os.path.join(tmp, "stock")] + list(extra) + args, check=True, stdout=subprocess.DEVNULL,
                    stderr=subprocess.DEVNULL, timeout=900)
-    env = dict(os.environ, T4_STREAMS="1", T4_BCSTATS="1", T4_SORT="1", T4_ANNOTATE="1")
+    env = dropin_env(binary, dict(T4_STREAMS="1", T4_BCSTATS="1", T4_SORT="1", T4_ANNOTATE="1"))
     r = subprocess.run([binary, "-t", "1", "-o", os.path.join(tmp, "dev")] + list(extra) + args, check=True, stdout=subprocess.DEVNULL,
                        stderr=subprocess.PIPE, timeout=900, env=env, text=True)
     assert "per-cell 21-mer statistics and barcode sort on the device" in r.stderr, r.stderr[-600:]
