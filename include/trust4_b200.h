@@ -439,6 +439,10 @@ int t4_mate_overlap_batch(const char *read_pool, size_t pool_bytes, const uint64
 /* Test hook, host only: SeqSet::LongestIncreasingSubsequence (SeqSet.hpp:342-474) exactly as the scan applies it to the
  * hits (a[i], b[i]) of a diagonal window sorted by b; returns the chain length, the chain in out_a / out_b (room for n). */
 int t4_test_lis(const int32_t *a, const int32_t *b, int n, int32_t *out_a, int32_t *out_b);
+/* Test hook: the main hit sort of GetOverlapsFromRead and its group / run head pass, on the device, over n 64-bit hit
+ * keys given in the order the probe emits them (scratch of the set s; the set is not changed).  out: the n keys
+ * sorted; heads: int32 {nG, nR, grp[0..nG], run[0..nR]} over the valid keys (room for 2 n + 4).  Returns n. */
+int t4_test_group_hits(t4_seqset *s, const uint64_t *keys, int n, uint64_t *out, int32_t *heads);
 /* The same on DEVICE buffers (ctrl: 64 bytes of device scratch; afterwards u64 ctrl[1] = reads with a hit, ctrl[2] =
  * low-complexity reads); n_workers CTAs (0 = one resident wave); asynchronous on cuda_stream. */
 int t4_refset_scan_device(t4_refset *r, const void *read_pool, const void *seq_off, const void *len, int64_t n,

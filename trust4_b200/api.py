@@ -37,7 +37,7 @@ EXPORTS = [
     "streams_assign_reads", "assign_free", "assign_results", "assign_stats", "assign_extended_set", "assign_device_buffers",
     "kmer_count_stats", "kmer_count_table_bytes", "kmer_count_stats_device", "kmer_count_table_stats",
     "refset_create_from_fa", "refset_free", "refset_size", "refset_name", "refset_seqset", "refset_set_hit_len_required",
-    "refset_set_radius", "refset_scan", "refset_scan_device", "test_lis", "test_check_eq_bytes", "refset_get_overlaps", "refset_annotate", "sort_reads", "mate_overlap_batch",
+    "refset_set_radius", "refset_scan", "refset_scan_device", "test_lis", "test_check_eq_bytes", "test_group_hits", "refset_get_overlaps", "refset_annotate", "sort_reads", "mate_overlap_batch",
     "barcode_kmer_count_stats", "barcode_kmer_count_stats_device", "sort_reads_barcode",
 ]
 
@@ -278,6 +278,21 @@ class SeqSet:
         if n < 0:
             self.lib.check(int(n))
         return int(n), int(bad.value)
+
+    def group_hits(self, keys):
+        """t4_test_group_hits: the device's main hit sort and head pass over 64-bit hit keys in emission order.
+        Returns (sorted keys, group heads, run heads), the heads over the valid keys and ending with their count."""
+        if not hasattr(self.lib, "test_group_hits"):
+            # resolved on first use, like check_eq_bytes
+            self.lib._f("test_group_hits", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p])
+        keys = np.ascontiguousarray(keys, dtype=np.uint64)
+        n = len(keys)
+        out = np.zeros(max(n, 1), np.uint64)
+        heads = np.zeros(2 * n + 4, np.int32)
+        r = self.lib.check(self.lib.test_group_hits(self.h, keys.ctypes.data, n, out.ctypes.data, heads.ctypes.data))
+        assert r == n
+        nG, nR = int(heads[0]), int(heads[1])
+        return out[:n], heads[2:3 + nG].astype(np.int64), heads[3 + nG:4 + nG + nR].astype(np.int64)
 
     def index_checksum(self):
         cs = C.c_uint64()

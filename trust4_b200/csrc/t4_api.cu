@@ -393,9 +393,9 @@ static int launch_ops( int kernel, T4Op *dOps, int n, void *stream )
 #if T4_CUDA
 	cudaStream_t cs = (cudaStream_t)stream ;
 	if ( kernel == T4K_STREAM )
-		t4_stream_kernel<<<n, E.nt, 0, cs>>>( E.A, dOps, E.gapTable ) ;
+		t4_stream_kernel<<<n, E.nt, T4_HIT_TILE_BYTES, cs>>>( E.A, dOps, E.gapTable ) ;
 	else if ( kernel == T4K_AUX )
-		t4_aux_kernel<<<n, E.nt, 0, cs>>>( E.A, dOps ) ;
+		t4_aux_kernel<<<n, E.nt, T4_HIT_TILE_BYTES, cs>>>( E.A, dOps ) ;
 	else
 		t4_annot_kernel<<<n, E.nt, 0, cs>>>( E.A, dOps ) ;
 	CK( cudaGetLastError() ) ;
@@ -582,6 +582,9 @@ int T4_API( init )( int device, size_t arena_bytes )
 		CK( cudaGetDevice( &device ) ) ;
 	CK( cudaSetDevice( device ) ) ;
 	CK( cudaDeviceGetAttribute( &E.sms, cudaDevAttrMultiProcessorCount, device ) ) ;
+	// the hit tile of c_get_overlaps (dynamic shared memory; with the static T4Smem it is more than 48 KB)
+	CK( cudaFuncSetAttribute( t4_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, T4_HIT_TILE_BYTES ) ) ;
+	CK( cudaFuncSetAttribute( t4_aux_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, T4_HIT_TILE_BYTES ) ) ;
 	if ( arena_bytes == 0 )
 	{
 		size_t fr = 0, tot = 0 ;
@@ -825,7 +828,8 @@ int T4_API( seqset_kmer_length )( t4_seqset *s )
 
 // run one op on one stream through the staging buffer.  extra: bytes copied in after the op record;
 // outBytes: bytes copied back from stage + outAt.
-static int run_single( T4Op &op, const void *extra, size_t extraBytes, size_t outAt, void *outHost, size_t outBytes, size_t totalStage )
+static int run_single( T4Op &op, const void *extra, size_t extraBytes, size_t outAt, void *outHost, size_t outBytes, size_t totalStage,
+	int kernel = T4K_STREAM )
 {
 	int r = ensure_stage( totalStage ) ;
 	if ( r ) return r ;
@@ -842,7 +846,7 @@ static int run_single( T4Op &op, const void *extra, size_t extraBytes, size_t ou
 		r = h2d( E.stage + sizeof( T4Op ), extra, extraBytes ) ;
 		if ( r ) return r ;
 	}
-	r = launch_ops( T4K_STREAM, (T4Op *)E.stage, 1, 0 ) ;
+	r = launch_ops( kernel, (T4Op *)E.stage, 1, 0 ) ;
 	if ( r ) return r ;
 	r = dsync() ;
 	if ( r ) return r ;
@@ -1308,6 +1312,35 @@ int64_t T4_API( seqset_index_checksum )( t4_seqset *s, uint64_t *checksum )
 	}
 	*checksum = sum ;
 	return total ;
+}
+
+// The main hit sort and head pass of GetOverlapsFromRead on given keys (test hook; the aux kernel runs it)
+int T4_API( test_group_hits )( t4_seqset *s, const uint64_t *keys, int n, uint64_t *out, int32_t *heads )
+{
+	int r = check( s ) ;
+	if ( r ) return r ;
+	if ( n < 0 || ( n && ( !keys || !out || !heads ) ) )
+	{
+		set_err( "t4_test_group_hits: bad arguments" ) ;
+		return T4_E_INVAL ;
+	}
+	const size_t keysAt = sizeof( T4Op ), outAt = keysAt + (size_t)n * 8, headsAt = outAt + (size_t)n * 8 ;
+	const size_t headsBytes = ( 2 * (size_t)n + 4 ) * 4 ;
+	T4Op op ;
+	memset( &op, 0, sizeof( op ) ) ;
+	op.streamOff = s->off ;
+	op.op = T4_OP_GROUP_HITS ;
+	op.read = keysAt ;
+	op.len = n ;
+	op.out = outAt ;
+	op.out2 = headsAt ;
+	r = run_single( op, keys, (size_t)n * 8, 0, 0, 0, headsAt + headsBytes + 64, T4K_AUX ) ;
+	if ( r ) return r ;
+	if ( op.ret < 0 )
+		return op.ret ;
+	if ( n && ( ( r = d2h( out, E.stage + outAt, (size_t)n * 8 ) ) || ( r = d2h( heads, E.stage + headsAt, headsBytes ) ) ) )
+		return r ;
+	return op.ret ;
 }
 
 // Every live column's equality byte against its posWeight counts (test hook of the t4_eq cache)

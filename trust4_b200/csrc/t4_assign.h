@@ -504,6 +504,9 @@ T4_D inline void c_run_aux_op( T4Ctx &cx, T4Op *op )
 		case T4_OP_ASSIGN:
 			c_assign_loop( cx, op ) ;
 			break ;
+		case T4_OP_GROUP_HITS:
+			c_test_group_hits( cx, op ) ;
+			break ;
 		case T4_OP_ASSIGN_RECOMPUTE:
 			c_assign_recompute( cx, op ) ;
 			break ;

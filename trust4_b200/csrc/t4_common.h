@@ -369,6 +369,7 @@ enum
 	T4_OP_ASSIGN_PREP,
 	T4_OP_ASSIGN,
 	T4_OP_ASSIGN_RECOMPUTE,
+	T4_OP_GROUP_HITS, // test hook t4_test_group_hits
 	// ... and the stage-0 scan against a reference gene set (t4_refscan.h)
 	T4_OP_REF_INPUT,
 	T4_OP_REF_SCAN,

@@ -1084,27 +1084,299 @@ T4_D inline u64 *c_sort_keys( T4Ctx &cx, u64 *a, u64 *b, u32 n )
 #endif
 }
 
-// Positions p in [0,n) where (keys[p] >> shift) differs from its predecessor's, in order; out[count] = n.
-T4_D inline u32 c_heads( T4Ctx &cx, const u64 *keys, u32 n, int shift, u32 *out )
+// ---------------------------------------------------------------------------
+// the main hit sort of GetOverlapsFromRead: a stable sort on the key prefix (strand | contig | diagonal)
+// ---------------------------------------------------------------------------
+// Up to T4_HIT_TILE keys are sorted and chained in dynamic shared memory (two buffers of T4_HIT_TILE + 1 keys; the
+// stream and aux kernels are launched with T4_HIT_TILE_BYTES of it), more in global memory.  No tile size costs
+// occupancy (the kernels stay register bound at 4 CTAs per SM), but the tile comes out of L1, through which the other
+// phases read contigs, postings and posWeight.  One default bench.py workload on an H100 80GB HBM3 (700 W), ms per
+// step against 583 for the parent's sort: a 2048-key tile 602, 1024 keys 565, 512 keys 556, no tile 556.
+#ifndef T4_HIT_TILE
+#define T4_HIT_TILE 512
+#endif
+#define T4_HIT_TILE_BYTES ( 2 * ( T4_HIT_TILE + 1 ) * 8 )
+#define T4_PREFIX_DIGIT 9 // widest radix digit: 2^9 counters per warp fill the radix area at 4 warps
+static_assert( T4_HIT_TILE <= T4_RADIX * T4_MAX_NT, "a run's hit length per run lives in the radix area" ) ;
+static_assert( ( 1 << T4_PREFIX_DIGIT ) * ( T4_MAX_NT / 32 ) <= T4_RADIX * T4_MAX_NT, "radix counters" ) ;
+#if T4_CUDA
+extern __shared__ __align__( 16 ) u64 t4_hit_tile[] ;
+#endif
+
+// The sorted hits as the chain pass reads them: keys (shared or global memory) and room for the group and run heads
+// (H + 1 each) and a hit length per run (H).
+struct T4HitView
+{
+	const u64 *keys ;
+	u32 *grp, *run, *hl ;
+} ;
+
+// Exclusive scans of two values per thread at once.
+T4_D inline void c_scan_threads2( T4Ctx &cx, u32 v0, u32 v1, u32 &o0, u32 &o1, u32 &t0, u32 &t1 )
+{
+#if T4_CUDA
+	const int lane = cx.tid & 31, warp = cx.tid >> 5, nwarps = cx.nt >> 5 ;
+	u32 i0 = v0, i1 = v1 ;
+#pragma unroll
+	for ( int d = 1 ; d < 32 ; d <<= 1 )
+	{
+		u32 x0 = __shfl_up_sync( 0xffffffffu, i0, d ) ;
+		u32 x1 = __shfl_up_sync( 0xffffffffu, i1, d ) ;
+		if ( lane >= d )
+		{
+			i0 += x0 ;
+			i1 += x1 ;
+		}
+	}
+	T4_SYNC() ;
+	if ( lane == 31 )
+	{
+		cx.sm->scan[warp] = i0 ;
+		cx.sm->scan[T4_MAX_NT / 32 + warp] = i1 ;
+	}
+	T4_SYNC() ;
+	u32 b0 = 0, b1 = 0, s0 = 0, s1 = 0 ;
+	for ( int w = 0 ; w < nwarps ; ++w )
+	{
+		u32 x0 = cx.sm->scan[w], x1 = cx.sm->scan[T4_MAX_NT / 32 + w] ;
+		if ( w < warp )
+		{
+			b0 += x0 ;
+			b1 += x1 ;
+		}
+		s0 += x0 ;
+		s1 += x1 ;
+	}
+	o0 = b0 + i0 - v0 ;
+	o1 = b1 + i1 - v1 ;
+	t0 = s0 ;
+	t1 = s1 ;
+#else
+	o0 = c_scan_threads( cx, v0, t0 ) ;
+	o1 = c_scan_threads( cx, v1, t1 ) ;
+#endif
+}
+
+// One neighbour-compare pass over the sorted keys: group heads (strand or contig changes) and run heads (the diagonal
+// changes too) in order, grp[nG] = run[nR] = n.  Every group head is a run head.
+T4_D inline void c_hit_heads( T4Ctx &cx, const u64 *keys, u32 n, u32 *grp, u32 *run, u32 &nG, u32 &nR )
 {
 	u32 chunk = ( n + cx.nt - 1 ) / cx.nt ;
 	u32 lo = cx.tid * chunk ;
 	u32 hi = lo + chunk < n ? lo + chunk : n ;
 	if ( lo > n )
 		lo = n ;
-	u32 c = 0 ;
+	u32 cg = 0, cr = 0 ;
+	u64 prev = lo > 0 && lo < hi ? keys[lo - 1] : 0 ;
 	for ( u32 i = lo ; i < hi ; ++i )
-		if ( i == 0 || ( keys[i] >> shift ) != ( keys[i - 1] >> shift ) )
-			++c ;
-	u32 total ;
-	u32 o = c_scan_threads( cx, c, total ) ;
+	{
+		u64 k = keys[i] ;
+		cg += i == 0 || ( k >> T4_KEY_IDX_SHIFT ) != ( prev >> T4_KEY_IDX_SHIFT ) ;
+		cr += i == 0 || ( k >> T4_KEY_C_SHIFT ) != ( prev >> T4_KEY_C_SHIFT ) ;
+		prev = k ;
+	}
+	u32 og, orr ;
+	c_scan_threads2( cx, cg, cr, og, orr, nG, nR ) ;
+	prev = lo > 0 && lo < hi ? keys[lo - 1] : 0 ;
 	for ( u32 i = lo ; i < hi ; ++i )
-		if ( i == 0 || ( keys[i] >> shift ) != ( keys[i - 1] >> shift ) )
-			out[o++] = i ;
+	{
+		u64 k = keys[i] ;
+		if ( i == 0 || ( k >> T4_KEY_IDX_SHIFT ) != ( prev >> T4_KEY_IDX_SHIFT ) )
+			grp[og++] = i ;
+		if ( i == 0 || ( k >> T4_KEY_C_SHIFT ) != ( prev >> T4_KEY_C_SHIFT ) )
+			run[orr++] = i ;
+		prev = k ;
+	}
 	if ( cx.tid == 0 )
-		out[total] = n ;
+	{
+		grp[nG] = n ;
+		run[nR] = n ;
+	}
 	T4_SYNC() ;
-	return total ;
+}
+
+#if T4_CUDA
+// Order-preserving map of a key's prefix onto few bits: (strand, contig - min contig, diagonal - min diagonal), each
+// field only as wide as its range over the read; invalid keys map above every valid one.
+struct T4PrefixRank
+{
+	u32 idxMin, cMin ;
+	int cb, sShift, tb ;
+
+	T4_D u64 operator()( u64 k ) const
+	{
+		if ( k == T4_KEY_INVALID )
+			return 1ull << tb ;
+		u64 r = ( (u64)( (u32)t4_key_idx( k ) - idxMin ) << cb ) | (u64)( (u32)( ( k >> T4_KEY_C_SHIFT ) & T4_KEY_C_MASK ) - cMin ) ;
+		if ( sShift >= 0 )
+			r |= ( k >> T4_KEY_STRAND_SHIFT ) << sShift ;
+		return r ;
+	}
+} ;
+
+T4_D inline int t4_bits( u32 x ) { return x ? 32 - __clz( x ) : 0 ; }
+#endif
+
+// Sorts the n keys of a[] (in c_get_hits' emission order) ascending and returns the global buffer holding them, a or
+// b, for scoring; *v says where the chain pass reads them and where it keeps its heads.
+//
+// The device sorts on the prefix key >> T4_KEY_C_SHIFT only, stably, and that gives the order of a sort on the whole
+// key: c_get_hits emits its hits in ascending (pass, q) order (the prefix sum and the serial walk both reserve slots
+// in q order, and a long list is copied into its own reserved slots), so within one (strand, contig, diagonal) the
+// hits come in ascending q, and b = q - c ascends with q.  Two hits never share (strand, contig, diagonal, b): the
+// diagonal and b fix q, and one position's postings are distinct (contig, offset) pairs, so the repeat flag (bit 0)
+// never breaks a tie.  Invalid keys (~0) sort last.  This does not hold for the other sorts (SortHits order, the
+// reference sets): they keep c_sort_keys.
+T4_D inline u64 *c_sort_hit_prefix( T4Ctx &cx, u64 *a, u64 *b, u32 n, T4HitView *v )
+{
+	T4Stream *st = cx.st ;
+#if !T4_CUDA
+	std::sort( a, a + n ) ;
+	v->keys = a ;
+	v->grp = cx.P<u32>( st->grpOff ) ;
+	v->run = cx.P<u32>( st->runOff ) ;
+	v->hl = (u32 *)b ;
+	return a ;
+#else
+	const bool tile = n <= T4_HIT_TILE ;
+	u64 *src = tile ? t4_hit_tile : a, *dst = tile ? t4_hit_tile + T4_HIT_TILE + 1 : b ;
+	{
+		// the ranges of the prefix fields; the tile is filled on the way
+		u32 iMin = ~0u, iMax = 0, cMin = ~0u, cMax = 0, sOr = 0, sAnd = 1, inv = 0 ;
+		for ( u32 i = cx.tid ; i < n ; i += cx.nt )
+		{
+			u64 k = a[i] ;
+			if ( tile )
+				src[i] = k ;
+			if ( k == T4_KEY_INVALID )
+			{
+				inv = 1 ;
+				continue ;
+			}
+			u32 ix = (u32)t4_key_idx( k ), c = (u32)( ( k >> T4_KEY_C_SHIFT ) & T4_KEY_C_MASK ), s = (u32)( k >> T4_KEY_STRAND_SHIFT ) ;
+			iMin = min( iMin, ix ) ;
+			iMax = max( iMax, ix ) ;
+			cMin = min( cMin, c ) ;
+			cMax = max( cMax, c ) ;
+			sOr |= s ;
+			sAnd &= s ;
+		}
+		const int lane = cx.tid & 31, warp = cx.tid >> 5, nwarps = cx.nt >> 5 ;
+		iMin = __reduce_min_sync( 0xffffffffu, iMin ) ;
+		iMax = __reduce_max_sync( 0xffffffffu, iMax ) ;
+		cMin = __reduce_min_sync( 0xffffffffu, cMin ) ;
+		cMax = __reduce_max_sync( 0xffffffffu, cMax ) ;
+		sOr = __reduce_or_sync( 0xffffffffu, sOr ) ;
+		sAnd = __reduce_and_sync( 0xffffffffu, sAnd ) ;
+		inv = __reduce_or_sync( 0xffffffffu, inv ) ;
+		T4_SYNC() ; // earlier readers of sm->scan are done
+		if ( lane == 0 )
+		{
+			u32 *w = cx.sm->scan + 7 * warp ;
+			w[0] = iMin ; w[1] = iMax ; w[2] = cMin ; w[3] = cMax ; w[4] = sOr ; w[5] = sAnd ; w[6] = inv ;
+		}
+		T4_SYNC() ;
+		for ( int x = 0 ; x < nwarps ; ++x )
+		{
+			const u32 *w = cx.sm->scan + 7 * x ;
+			iMin = min( iMin, w[0] ) ; iMax = max( iMax, w[1] ) ; cMin = min( cMin, w[2] ) ; cMax = max( cMax, w[3] ) ;
+			sOr |= w[4] ; sAnd &= w[5] ; inv |= w[6] ;
+		}
+		const bool anyValid = iMin <= iMax ;
+		T4PrefixRank rank ;
+		rank.idxMin = iMin ;
+		rank.cMin = cMin ;
+		rank.cb = anyValid ? t4_bits( cMax - cMin ) : 0 ;
+		const int ib = anyValid ? t4_bits( iMax - iMin ) : 0 ;
+		const int sb = ( anyValid && sOr != sAnd ) ? 1 : 0 ;
+		rank.sShift = sb ? rank.cb + ib : -1 ;
+		rank.tb = rank.cb + ib + sb ;
+		const int nb = rank.tb + (int)inv ;
+		// LSD radix over the rank in digits of equal width (at most T4_PREFIX_DIGIT bits), one contiguous chunk of keys
+		// per warp; lanes with equal digits find each other with __match_any_sync and rank themselves by lane, so the
+		// scatter is stable.  Counters: digit-major, warp-minor, in the radix area.
+		const int passes = ( nb + T4_PREFIX_DIGIT - 1 ) / T4_PREFIX_DIGIT ;
+		const int width = passes ? ( nb + passes - 1 ) / passes : 0 ;
+		const u32 D = 1u << width ;
+		const u32 wchunk = ( ( n + nwarps - 1 ) / nwarps + 31 ) & ~31u ;
+		const u32 wlo = warp * wchunk < n ? warp * wchunk : n ;
+		const u32 whi = wlo + wchunk < n ? wlo + wchunk : n ;
+		const unsigned lt = ( 1u << lane ) - 1u ;
+		u32 *cnt = cx.sm->radix ;
+		for ( int shift = 0 ; shift < nb ; shift += width )
+		{
+			for ( u32 x = cx.tid ; x < D * nwarps ; x += cx.nt )
+				cnt[x] = 0 ;
+			T4_SYNC() ;
+			for ( u32 i0 = wlo ; i0 < whi ; i0 += 32 )
+			{
+				u32 i = i0 + lane ;
+				bool have = i < whi ;
+				u32 d = have ? (u32)( rank( src[i] ) >> shift ) & ( D - 1 ) : D + lane ; // idle lanes: private pseudo digits
+				unsigned peers = __match_any_sync( 0xffffffffu, d ) ;
+				if ( have && ( peers & lt ) == 0 )
+					cnt[d * nwarps + warp] += __popc( peers ) ;
+				__syncwarp() ;
+			}
+			T4_SYNC() ;
+			{
+				const int total = (int)D * nwarps ;
+				const int per = ( total + cx.nt - 1 ) / cx.nt ;
+				const int lo2 = cx.tid * per < total ? cx.tid * per : total ;
+				const int hi2 = lo2 + per < total ? lo2 + per : total ;
+				u32 sum = 0 ;
+				for ( int x = lo2 ; x < hi2 ; ++x )
+					sum += cnt[x] ;
+				u32 tot ;
+				u32 base = c_scan_threads( cx, sum, tot ) ;
+				for ( int x = lo2 ; x < hi2 ; ++x )
+				{
+					u32 c = cnt[x] ;
+					cnt[x] = base ;
+					base += c ;
+				}
+			}
+			T4_SYNC() ;
+			for ( u32 i0 = wlo ; i0 < whi ; i0 += 32 )
+			{
+				u32 i = i0 + lane ;
+				bool have = i < whi ;
+				u64 k = have ? src[i] : 0 ;
+				u32 d = have ? (u32)( rank( k ) >> shift ) & ( D - 1 ) : D + lane ;
+				unsigned peers = __match_any_sync( 0xffffffffu, d ) ;
+				u32 pos = 0 ;
+				if ( have )
+					pos = cnt[d * nwarps + warp] + __popc( peers & lt ) ;
+				__syncwarp() ;
+				if ( have )
+				{
+					dst[pos] = k ;
+					if ( ( peers & lt ) == 0 )
+						cnt[d * nwarps + warp] += __popc( peers ) ;
+				}
+				__syncwarp() ;
+			}
+			T4_SYNC() ;
+			u64 *t = src ; src = dst ; dst = t ;
+		}
+	}
+	v->keys = src ;
+	if ( !tile )
+	{
+		v->grp = cx.P<u32>( st->grpOff ) ;
+		v->run = cx.P<u32>( st->runOff ) ;
+		v->hl = (u32 *)dst ;
+		return src ;
+	}
+	// scoring reads the keys after the tile is gone: one coalesced copy out.  The other buffer holds the heads
+	// (2 n + 2 <= 2 T4_HIT_TILE + 2 words), the radix area the hit lengths.
+	for ( u32 i = cx.tid ; i < n ; i += cx.nt )
+		a[i] = src[i] ;
+	v->run = (u32 *)dst ;
+	v->grp = (u32 *)dst + n + 1 ;
+	v->hl = cx.sm->radix ;
+	return a ;
+#endif
 }
 
 // ---------------------------------------------------------------------------
@@ -1713,20 +1985,22 @@ T4_D inline u32 c_get_hits( T4Ctx &cx, int len, int strand, int barcode, bool al
 // diagonal; on one diagonal b and a increase together, hence LongestIncreasingSubsequence (SeqSet.hpp:342)
 // returns its input unchanged and the chain IS the run.  GetVJOverlapsFromHits only ever sees isRef hits.
 //
-// keys: sorted, H valid hits.  tmp: spare u64[H].  keysR (may be 0): the same hits sorted in SortHits order
+// v: the sorted hits (c_sort_hit_prefix), H valid.  keysR (may be 0): the same hits sorted in SortHits order
 // (strand, idx, a, b) -- only needed to reproduce the `hits[k].repeats` indexing of SeqSet.hpp:931-947 when
 // some k-mer has more than 10000 postings.
-T4_D inline int c_overlaps_from_hits( T4Ctx &cx, const u64 *keys, u32 H, u64 *tmp, const u64 *keysR, int hitLenRequired,
+T4_D inline int c_overlaps_from_hits( T4Ctx &cx, const T4HitView &v, u32 H, const u64 *keysR, int hitLenRequired,
 	int filter )
 {
 	T4Stream *st = cx.st ;
 	T4Smem *sm = cx.sm ;
 	const int k = st->kmerLength ;
-	u32 *grp = cx.P<u32>( st->grpOff ) ;
-	u32 *run = cx.P<u32>( st->runOff ) ;
-	u32 nG = c_heads( cx, keys, H, T4_KEY_IDX_SHIFT, grp ) ;
-	u32 nR = c_heads( cx, keys, H, T4_KEY_C_SHIFT, run ) ;
-	// pre-pass (SeqSet.hpp:781-824), including its group-skipping loop increment
+	const u64 *keys = v.keys ;
+	u32 *grp = v.grp ;
+	u32 *run = v.run ;
+	u32 *hl = v.hl ;
+	u32 nG, nR ;
+	c_hit_heads( cx, keys, H, grp, run, nG, nR ) ;
+	// pre-pass (SeqSet.hpp:781-824), including its group-skipping loop increment, over the group heads
 	if ( cx.tid == 0 )
 	{
 		int novelMin[2] = {3, 3} ;
@@ -1783,29 +2057,33 @@ T4_D inline int c_overlaps_from_hits( T4Ctx &cx, const u64 *keys, u32 H, u64 *tm
 	int novelMin[2] = { sm->bi[0], sm->bi[1] } ;
 	int removeOnlyRepeats[2] = { sm->bi[2], sm->bi[3] } ;
 	T4_SYNC() ;
-	// one candidate per diagonal run (SeqSet.hpp:906-1057)
+	// one candidate per diagonal run (SeqSet.hpp:906-1057).  Every test below only rejects, so their order is free: the
+	// cheap ones first.  The reference's test of the group size (< minHit) is implied by the run's, as the run lies
+	// inside its group.
 	for ( u32 r = cx.tid ; r < nR ; r += cx.nt )
 	{
 		u32 s = run[r], e = run[r + 1] ;
+		hl[r] = 0 ;
+		int n = (int)( e - s ) ;
+		if ( n * k < hitLenRequired )
+			continue ;
 		u64 k0 = keys[s] ;
 		int plus = (int)( k0 >> T4_KEY_STRAND_SHIFT ) ;
-		int minHit = novelMin[plus] ;
-		tmp[r] = 0 ;
-		// group [gi, gj) containing this run
-		u32 lo = 0, hi = nG ;
-		while ( hi - lo > 1 )
-		{
-			u32 mid = ( lo + hi ) / 2 ;
-			if ( grp[mid] <= s )
-				lo = mid ;
-			else
-				hi = mid ;
-		}
-		u32 gi = grp[lo], gj = grp[lo + 1] ;
-		if ( (int)( gj - gi ) < minHit )
+		if ( n < novelMin[plus] )
 			continue ;
 		if ( removeOnlyRepeats[plus] && keysR != 0 )
 		{
+			// group [gi, gj) containing this run
+			u32 lo = 0, hi = nG ;
+			while ( hi - lo > 1 )
+			{
+				u32 mid = ( lo + hi ) / 2 ;
+				if ( grp[mid] <= s )
+					lo = mid ;
+				else
+					hi = mid ;
+			}
+			u32 gi = grp[lo], gj = grp[lo + 1] ;
 			bool hasUnique = false ;
 			for ( u32 x = gi ; x < gj ; ++x )
 				if ( !t4_key_big( keysR[x] ) )
@@ -1815,14 +2093,8 @@ T4_D inline int c_overlaps_from_hits( T4Ctx &cx, const u64 *keys, u32 H, u64 *tm
 				}
 			if ( !hasUnique )
 				continue ;
-		}
-		int n = (int)( e - s ) ;
-		if ( n < minHit || n * k < hitLenRequired )
-			continue ;
-		if ( removeOnlyRepeats[plus] && keysR != 0 )
-		{
 			// SeqSet.hpp:931-947 indexes hits[] with the run-local range [s - gi, e - gi)
-			bool hasUnique = false ;
+			hasUnique = false ;
 			for ( u32 x = s - gi ; x < e - gi ; ++x )
 				if ( !t4_key_big( keysR[x] ) )
 				{
@@ -1832,8 +2104,6 @@ T4_D inline int c_overlaps_from_hits( T4Ctx &cx, const u64 *keys, u32 H, u64 *tm
 			if ( !hasUnique )
 				continue ;
 		}
-		if ( n * k < hitLenRequired ) // lisSize * kmerLength (SeqSet.hpp:966)
-			continue ;
 		// GetTotalHitLengthOnRead / OnSeq (SeqSet.hpp:3330, 3352): identical on a single diagonal
 		int hitLen = 0 ;
 		{
@@ -1860,7 +2130,7 @@ T4_D inline int c_overlaps_from_hits( T4Ctx &cx, const u64 *keys, u32 H, u64 *tm
 		int seqEnd = t4_key_b( keys[e - 1] ) + k - 1 ;
 		if ( hitLen * 2 < seqEnd - seqStart + 1 )
 			continue ;
-		tmp[r] = (u64)hitLen ;
+		hl[r] = (u32)hitLen ;
 	}
 	T4_SYNC() ;
 	// compact the kept runs, in key order, into overlaps
@@ -1871,7 +2141,7 @@ T4_D inline int c_overlaps_from_hits( T4Ctx &cx, const u64 *keys, u32 H, u64 *tm
 		lo = nR ;
 	u32 c = 0 ;
 	for ( u32 r = lo ; r < hi ; ++r )
-		if ( tmp[r] )
+		if ( hl[r] )
 			++c ;
 	u32 total ;
 	u32 o = c_scan_threads( cx, c, total ) ;
@@ -1881,10 +2151,10 @@ T4_D inline int c_overlaps_from_hits( T4Ctx &cx, const u64 *keys, u32 H, u64 *tm
 	T4Ovl *ovl = cx.P<T4Ovl>( st->ovlOff ) ;
 	for ( u32 r = lo ; r < hi ; ++r )
 	{
-		if ( !tmp[r] )
+		if ( !hl[r] )
 			continue ;
 		u32 s = run[r], e = run[r + 1] ;
-		int hitLen = (int)tmp[r] ;
+		int hitLen = (int)hl[r] ;
 		T4Ovl no ;
 		no.seqIdx = t4_key_idx( keys[s] ) ;
 		no.readStart = t4_key_a( keys[s] ) ;
@@ -1903,6 +2173,47 @@ T4_D inline int c_overlaps_from_hits( T4Ctx &cx, const u64 *keys, u32 H, u64 *tm
 	}
 	T4_SYNC() ;
 	return (int)total ;
+}
+
+// Test hook t4_test_group_hits: c_sort_hit_prefix and c_hit_heads over op->len keys given at op->read, in emission
+// order.  The sorted keys go to op->out, {nG, nR, grp[0..nG], run[0..nR]} over the valid keys to op->out2.
+T4_D inline void c_test_group_hits( T4Ctx &cx, T4Op *op )
+{
+	T4Stream *st = cx.st ;
+	const u32 n = (u32)op->len ;
+	c_ensure_hits( cx, n ) ;
+	if ( st->error )
+		return ;
+	u64 *a = cx.P<u64>( st->keysAOff ) ;
+	u64 *b = cx.P<u64>( st->keysBOff ) ;
+	const u64 *in = t4_x<u64>( op->read ) ;
+	for ( u32 i = cx.tid ; i < n ; i += cx.nt )
+		a[i] = in[i] ;
+	T4_SYNC() ;
+	T4HitView v ;
+	const u64 *sorted = c_sort_hit_prefix( cx, a, b, n, &v ) ;
+	u32 c = 0 ;
+	for ( u32 i = cx.tid ; i < n ; i += cx.nt )
+		if ( v.keys[i] != T4_KEY_INVALID )
+			++c ;
+	u32 H ;
+	c_scan_threads( cx, c, H ) ;
+	u32 nG, nR ;
+	c_hit_heads( cx, v.keys, H, v.grp, v.run, nG, nR ) ;
+	u64 *out = t4_x<u64>( op->out ) ;
+	int32_t *heads = t4_x<int32_t>( op->out2 ) ;
+	for ( u32 i = cx.tid ; i < n ; i += cx.nt )
+		out[i] = sorted[i] ;
+	for ( u32 i = cx.tid ; i <= nG ; i += cx.nt )
+		heads[2 + i] = (int32_t)v.grp[i] ;
+	for ( u32 i = cx.tid ; i <= nR ; i += cx.nt )
+		heads[3 + nG + i] = (int32_t)v.run[i] ;
+	if ( cx.tid == 0 )
+	{
+		heads[0] = (int32_t)nG ;
+		heads[1] = (int32_t)nR ;
+		op->ret = (int)n ;
+	}
 }
 
 // `_overlap::operator<` (SeqSet.hpp:104-128)
@@ -2042,22 +2353,21 @@ T4_D T4_BIG int c_get_overlaps( T4Ctx &cx, int len, int strand, int barcode, boo
 			T4_SYNC() ;
 			keysR = c_sort_keys( cx, ra, rb, H ) ;
 		}
-		u64 *sorted = c_sort_keys( cx, a, b, H ) ;
+		T4HitView v ;
+		keys = c_sort_hit_prefix( cx, a, b, H, &v ) ;
 		// invalid keys (barcode filter) sorted to the end
 		if ( barcode != -1 )
 		{
 			u32 c = 0 ;
 			for ( u32 i = cx.tid ; i < H ; i += cx.nt )
-				if ( sorted[i] != T4_KEY_INVALID )
+				if ( v.keys[i] != T4_KEY_INVALID )
 					++c ;
 			u32 total ;
 			c_scan_threads( cx, c, total ) ;
 			H = total ;
 		}
-		keys = sorted ;
-		u64 *tmp = ( sorted == a ) ? b : a ;
 		T4_PHASE( cx, 3 ) ;
-		overlapCnt = c_overlaps_from_hits( cx, sorted, H, tmp, keysR, st->hitLenRequired, pass == 0 ? 0 : 1 ) ;
+		overlapCnt = c_overlaps_from_hits( cx, v, H, keysR, st->hitLenRequired, pass == 0 ? 0 : 1 ) ;
 		if ( st->error )
 			return 0 ;
 	}
