@@ -4,8 +4,9 @@ Runs R rounds, alternating the builds (A B, B A, A B, ...) so that drift of the 
 
     bench.py --no-cpu-baseline --dump-outputs <tmp>/<build><round> [extra bench args]
 
-each build selected through T4_LIB_PATH, and prints per run ms_per_step, roofline.phase_share, extend_split,
-per_read and stream_balance, plus the stream kernel's device counters of the run (bench.py's kernel-only launch).
+each build selected through T4_LIB_PATH, and prints per run ms_per_step, the AssignRead pass's time (assign_pass.ms),
+roofline.phase_share, extend_split, per_read and stream_balance, plus the stream kernel's device counters of the run
+(bench.py's kernel-only launch).
 Then it checks that every dumped .npy is byte-identical across all runs of both builds.
 
     python bench/ab_compare.py --build-parent HEAD       # cross-compile the parent into bench/_parent/ (git-ignored)
@@ -117,7 +118,8 @@ def main():
                 d = os.path.join(tmp, "%s%d" % (name, r))
                 line, ctr = run_one(path, d, args.bench_args)
                 rl = line["roofline"]
-                run = {"build": name, "round": r, "ms_per_step": line["ms_per_step"], "phase_share": rl["phase_share"],
+                run = {"build": name, "round": r, "ms_per_step": line["ms_per_step"],
+                       "assign_ms": (line.get("assign_pass") or {}).get("ms"), "phase_share": rl["phase_share"],
                        "extend_split": rl["extend_split"], "per_read": rl["per_read"], "stream_balance": rl["stream_balance"],
                        "counters": ctr, "dump": d}
                 if ctr and ctr["reads"] > 0:
@@ -127,10 +129,12 @@ def main():
         names, bad = same_outputs([x["dump"] for x in runs])
 
     ms = {b: [x["ms_per_step"] for x in runs if x["build"] == b] for b in ("A", "B")}
+    ams = {b: [x["assign_ms"] for x in runs if x["build"] == b and x["assign_ms"] is not None] for b in ("A", "B")}
     summary = {"a": args.a, "b": args.b, "rounds": args.rounds,
                "ms_per_step": ms, "median_ms": {b: float(np.median(v)) for b, v in ms.items()},
                "b_vs_a_median": float(np.median(ms["B"]) / np.median(ms["A"]) - 1.0),
                "every_b_below_every_a": max(ms["B"]) < min(ms["A"]),
+               "assign_ms": ams, "assign_median_ms": {b: float(np.median(v)) if v else None for b, v in ams.items()},
                "outputs_compared": names, "outputs_identical": not bad, "output_differences": bad}
     print("AB_SUMMARY " + json.dumps(summary), flush=True)
     if args.out:

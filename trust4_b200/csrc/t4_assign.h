@@ -226,7 +226,7 @@ T4_D inline void c_assign_prep( T4Ctx &cx, T4Op *op )
 
 // ---- ASSIGN ------------------------------------------------------------------------------------------------------
 // int SeqSet::AssignRead( read, strand, barcode, assign ), SeqSet.hpp:4632-4702, novel-contig set.  Collective; the read
-// is in cx.sm->read / rc.  Returns the contig slot (result in cx.sm->e0) or -1.
+// is in cx.sm->read / rc.  Returns the contig slot (result in cx.sm->plan.e0) or -1.
 T4_D inline int c_assign_read( T4Ctx &cx, int len, int strand, int barcode )
 {
 	T4Stream *st = cx.st ;
@@ -239,43 +239,10 @@ T4_D inline int c_assign_read( T4Ctx &cx, int len, int strand, int barcode )
 	T4Ovl *overlaps = cx.P<T4Ovl>( st->ovlOff ) ;
 	const char *r = ( overlaps[0].strand == 1 ) ? sm->read : sm->rc ;
 	const double factor = barcode == -1 ? 1.0 : 2.0 ; // SeqSet.hpp:4678
-	// ExtendOverlap is a pure function of (overlap, read, contig): all overlaps at once, then the first in order that
-	// extends over the whole read wins (SeqSet.hpp:4674-4690)
-	u32 *bits = cx.P<u32>( st->bitsOff ) ;
-	c_overhang_bits( cx, overlaps, overlapCnt, r, len, bits ) ;
-	T4SideStats *sstats = (T4SideStats *)cx.P<char>( st->failOff ) ;
-	T4DpScratch ds = t4_dp_scratch( cx ) ;
-	T4_PAR_FOR( x, 2 * overlapCnt )
-	{
-		const int i = x >> 1, right = x & 1 ;
-		const T4Ovl &o = overlaps[i] ;
-		T4Contig *seq = t4_seq( cx, o.seqIdx ) ;
-		int *pw = t4_pw( cx, seq ) ;
-		T4AlignView av ;
-		if ( !right )
-		{
-			int L = t4_min( o.readStart, o.seqStart ) ;
-			av = t4_overhang_align( pw + 4 * ( o.seqStart - L ), r + o.readStart - L, L, bits + 32 * i, ds ) ;
-		}
-		else
-		{
-			int R = t4_min( len - 1 - o.readEnd, seq->len - 1 - o.seqEnd ) ;
-			av = t4_overhang_align( pw + 4 * ( o.seqEnd + 1 ), r + o.readEnd + 1, R, bits + 32 * i + 16, ds ) ;
-		}
-		if ( av.dp )
-			t4_count( cx, 1, 1 ) ;
-		sstats[x] = t4_side_stats( av, !right ) ;
-	}
-	T4_SYNC() ;
+	// ExtendOverlap of every overlap, all exact (no similarity reaches 2), then the first in order that extends over the
+	// whole read wins (SeqSet.hpp:4674-4690)
 	T4Ovl *pre = cx.P<T4Ovl>( st->extOff ) ;
-	T4_PAR_FOR( i, overlapCnt )
-	{
-		T4Ovl e ;
-		int ok = t4_extend_finish( cx, len, t4_seq( cx, overlaps[i].seqIdx ), factor, overlaps[i], e, sstats[2 * i], sstats[2 * i + 1] ) ;
-		e.infoFromHits = ok ;
-		pre[i] = e ;
-	}
-	T4_SYNC() ;
+	c_extend_overlaps( cx, overlaps, overlapCnt, r, len, factor, 2.0, pre, 0 ) ;
 	if ( cx.tid == 0 )
 	{
 		int i ;
@@ -284,12 +251,11 @@ T4_D inline int c_assign_read( T4Ctx &cx, int len, int strand, int barcode )
 				break ;
 		if ( i < overlapCnt )
 		{
-			sm->e0 = pre[i] ;
+			sm->plan.e0 = pre[i] ;
 			sm->bi[0] = pre[i].seqIdx ;
 		}
 		else
 			sm->bi[0] = -1 ;
-		t4_count( cx, 16, (u64)overlapCnt ) ;
 	}
 	T4_SYNC() ;
 	const int ret = sm->bi[0] ;
@@ -367,7 +333,7 @@ T4_D inline void c_assign_loop( T4Ctx &cx, T4Op *op )
 			if ( failed )
 				break ;
 			// the result goes to this record and to the neighbours that share it (a contiguous range of slots)
-			const T4Ovl e = sm->e0 ;
+			const T4Ovl e = sm->plan.e0 ;
 			const i64 hi = descOff[j + 1] ;
 			for ( i64 p = s + cx.tid ; p < hi && leader[p] == (int32_t)s ; p += cx.nt )
 			{

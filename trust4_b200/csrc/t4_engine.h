@@ -39,6 +39,19 @@
 #define SCORE_MISMATCH (-2)
 #define SCORE_INDEL (-4)
 
+// What AddRead's decision walk and merge commit (thread 0) hand its collective phases (c_add_read).  kind: 0 nothing
+// to commit, 1 extend / inside the contig of e0, 2 merged (the merge is done).  AssignRead's result is e0 as well.
+struct T4AddPlan
+{
+	T4Ovl e0 ;
+	int kind ;
+	int seqIdx ;
+	int readInConsensusOffset ;
+	int ret ;
+	bool bail ;
+	bool added ;
+} ;
+
 struct T4Smem
 {
 	char read[T4_DEV_MAX_READ + 8] ;
@@ -50,7 +63,7 @@ struct T4Smem
 	u64 red[2] ;
 	u64 icode[T4_IDX_CHUNK] ; // c_index_op: k-mer codes of the current chunk of positions
 	unsigned char iact[T4_IDX_CHUNK] ;
-	T4Ovl e0 ;             // commit plan of c_add_read
+	T4AddPlan plan ;
 	u32 wnib[T4_MAX_NT / 32][2][64] ;        // per warp, per overhang side: IsBaseEqual nibbles of up to 512 columns
 	u32 wbits[T4_MAX_NT / 32][2][16] ;       // ... and the match bits against the read
 	u32 wact[T4_MAX_NT / 32][2][13 * T4_WACT_WORDS] ; // ... traceback words of the half-warp DP (n <= 16*T4_WACT_WORDS - 1)
@@ -2614,14 +2627,37 @@ T4_D inline T4SideStats t4_side_stats( const T4AlignView &av, bool fromEnd )
 	return r ;
 }
 
+// One overhang side of ExtendOverlap (SeqSet.hpp:1165-1175): n columns from contig column col against read positions
+// rp .. rp + n - 1.  The only place that derives a side from an overlap.
+struct T4Side { int n, col, rp ; } ;
+
+// Side `right` (0 left, 1 right) of overlap o of a read of length len against a contig of length seqLen.
+T4_HD inline T4Side t4_overhang_side( const T4Ovl &o, int right, int len, int seqLen )
+{
+	T4Side s ;
+	if ( !right )
+	{
+		s.n = t4_min( o.readStart, o.seqStart ) ;
+		s.col = o.seqStart - s.n ;
+		s.rp = o.readStart - s.n ;
+	}
+	else
+	{
+		s.n = t4_min( len - 1 - o.readEnd, seqLen - 1 - o.seqEnd ) ;
+		s.col = o.seqEnd + 1 ;
+		s.rp = o.readEnd + 1 ;
+	}
+	return s ;
+}
+
 // The rest of ExtendOverlap (SeqSet.hpp:1226-1277) given both sides' statistics.
 T4_D inline int t4_extend_finish( T4Ctx &cx, int len, T4Contig *seq, double mismatchThresholdFactor, const T4Ovl &overlap, T4Ovl &ext,
 	const T4SideStats &ls, const T4SideStats &rs )
 {
 	T4Stream *st = cx.st ;
 	int ret = 1 ;
-	int leftOverhangSize = t4_min( overlap.readStart, overlap.seqStart ) ;
-	int rightOverhangSize = t4_min( len - 1 - overlap.readEnd, seq->len - 1 - overlap.seqEnd ) ;
+	int leftOverhangSize = t4_overhang_side( overlap, 0, len, seq->len ).n ;
+	int rightOverhangSize = t4_overhang_side( overlap, 1, len, seq->len ).n ;
 	int matchCnt = ls.m + rs.m, mismatchCnt = ls.x + rs.x ;
 	if ( ls.ind > 0 )
 	{
@@ -2672,19 +2708,17 @@ T4_D inline int t4_extend_finish( T4Ctx &cx, int len, T4Contig *seq, double mism
 T4_D inline int t4_extend_overlap( T4Ctx &cx, const char *r, int len, T4Contig *seq, double mismatchThresholdFactor,
 	T4DpScratch &ds, const T4Ovl &overlap, T4Ovl &ext, const u32 *lbits, const u32 *rbits )
 {
-	int leftOverhangSize = t4_min( overlap.readStart, overlap.seqStart ) ;
-	int rightOverhangSize = t4_min( len - 1 - overlap.readEnd, seq->len - 1 - overlap.seqEnd ) ;
+	const T4Side L = t4_overhang_side( overlap, 0, len, seq->len ), R = t4_overhang_side( overlap, 1, len, seq->len ) ;
 	int *pw = t4_pw( cx, seq ) ;
 	T4SideStats ls, rs ;
 	{
-		T4AlignView av = t4_overhang_align( pw + 4 * ( overlap.seqStart - leftOverhangSize ), r + overlap.readStart - leftOverhangSize,
-			leftOverhangSize, lbits, ds ) ;
+		T4AlignView av = t4_overhang_align( pw + 4 * L.col, r + L.rp, L.n, lbits, ds ) ;
 		if ( av.dp )
 			t4_count( cx, 1, 1 ) ;
 		ls = t4_side_stats( av, true ) ;
 	}
 	{
-		T4AlignView av = t4_overhang_align( pw + 4 * ( overlap.seqEnd + 1 ), r + overlap.readEnd + 1, rightOverhangSize, rbits, ds ) ;
+		T4AlignView av = t4_overhang_align( pw + 4 * R.col, r + R.rp, R.n, rbits, ds ) ;
 		if ( av.dp )
 			t4_count( cx, 1, 1 ) ;
 		rs = t4_side_stats( av, false ) ;
@@ -3617,17 +3651,11 @@ T4_D inline int t4_side_span( T4Ctx &cx, const T4Ovl &o, int right, const char *
 	const unsigned char **te, const char **p )
 {
 	T4Contig *seq = t4_seq( cx, o.seqIdx ) ;
-	const int col = right ? o.seqEnd + 1 : o.seqStart - t4_min( o.readStart, o.seqStart ) ;
-	*tw = t4_pw( cx, seq ) + 4 * col ;
-	*te = t4_eq( cx, seq ) + col ;
-	if ( !right )
-	{
-		int L = t4_min( o.readStart, o.seqStart ) ;
-		*p = r + o.readStart - L ;
-		return L ;
-	}
-	*p = r + o.readEnd + 1 ;
-	return t4_min( len - 1 - o.readEnd, seq->len - 1 - o.seqEnd ) ;
+	const T4Side s = t4_overhang_side( o, right, len, seq->len ) ;
+	*tw = t4_pw( cx, seq ) + 4 * s.col ;
+	*te = t4_eq( cx, seq ) + s.col ;
+	*p = r + s.rp ;
+	return s.n ;
 }
 
 // ExtendOverlap's overhang alignments of the sides pend[0 .. cnt) (each needs the banded DP): their statistics into
@@ -3709,10 +3737,10 @@ T4_D inline u32 w_overhang_masks( T4Ctx &cx, const T4Ovl &o, const char *r, int 
 {
 	T4Contig *seq = t4_seq( cx, o.seqIdx ) ;
 	const unsigned char *eq = t4_eq( cx, seq ) ;
-	const int L = t4_min( o.readStart, o.seqStart ) ;
-	const int R = t4_min( len - 1 - o.readEnd, seq->len - 1 - o.seqEnd ) ;
-	const unsigned char *eL = eq + o.seqStart - L, *eR = eq + o.seqEnd + 1 ;
-	const char *pL = r + o.readStart - L, *pR = r + o.readEnd + 1 ;
+	const T4Side sL = t4_overhang_side( o, 0, len, seq->len ), sR = t4_overhang_side( o, 1, len, seq->len ) ;
+	const int L = sL.n, R = sR.n ;
+	const unsigned char *eL = eq + sL.col, *eR = eq + sR.col ;
+	const char *pL = r + sL.rp, *pR = r + sR.rp ;
 	const int nw = ( t4_max( L, R ) + 31 ) >> 5 ;
 	u32 mine = 0 ;
 	for ( int w0 = 0 ; w0 < nw ; w0 += 8 )
@@ -3745,50 +3773,30 @@ T4_D inline u32 w_overhang_masks( T4Ctx &cx, const T4Ovl &o, const char *r, int 
 
 // IsBaseEqual( column, read base ) of every overhang column of every overlap (ExtendOverlap, SeqSet.hpp:1165-1175) as bit
 // masks: bits[32 * i + 16 * side + w] holds overhang positions 32 w .. 32 w + 31 of side (0 left, 1 right) of overlap i.
-// Collective; r is the read in the strand of the overlaps.
+// Collective; r is the read in the strand of the overlaps.  The emulation's form of w_overhang_masks.
+#if !T4_CUDA
 T4_D inline void c_overhang_bits( T4Ctx &cx, const T4Ovl *overlaps, int overlapCnt, const char *r, int len, u32 *bits )
 {
-#if T4_CUDA
-	const int warp = cx.tid >> 5, nwarps = cx.nt >> 5, lane = cx.tid & 31 ;
-	for ( int oi = warp ; oi < overlapCnt ; oi += nwarps )
-	{
-		const T4Ovl o = overlaps[oi] ;
-		int nL, nR ;
-		bits[32 * oi + lane] = w_overhang_masks( cx, o, r, len, lane, &nL, &nR ) ;
-	}
-#else
 	T4_PAR_FOR( x, overlapCnt * 32 )
 	{
 		int oi = x >> 5, w = x & 15, right = ( x >> 4 ) & 1 ;
 		const T4Ovl &o = overlaps[oi] ;
 		T4Contig *seq = t4_seq( cx, o.seqIdx ) ;
-		int n, col0, rp0 ;
-		if ( !right )
-		{
-			n = t4_min( o.readStart, o.seqStart ) ;
-			col0 = o.seqStart - n ;
-			rp0 = o.readStart - n ;
-		}
-		else
-		{
-			n = t4_min( len - 1 - o.readEnd, seq->len - 1 - o.seqEnd ) ;
-			col0 = o.seqEnd + 1 ;
-			rp0 = o.readEnd + 1 ;
-		}
+		const T4Side s = t4_overhang_side( o, right, len, seq->len ) ;
 		u32 m = 0 ;
-		if ( w * 32 < n )
+		if ( w * 32 < s.n )
 		{
 			const unsigned char *eq = t4_eq( cx, seq ) ;
-			int hi = n - w * 32 < 32 ? n - w * 32 : 32 ;
+			int hi = s.n - w * 32 < 32 ? s.n - w * 32 : 32 ;
 			for ( int t = 0 ; t < hi ; ++t )
-				if ( t4_eq_hit( eq[col0 + w * 32 + t], r[rp0 + w * 32 + t] ) )
+				if ( t4_eq_hit( eq[s.col + w * 32 + t], r[s.rp + w * 32 + t] ) )
 					m |= 1u << t ;
 		}
 		bits[x] = m ;
 	}
-#endif
 	T4_SYNC() ;
 }
+#endif
 
 // Lazy ExtendOverlap: pre[i] of c_add_read from the statistics of overlap i's two sides (ind == -1: deferred to the
 // banded DP).  With both sides settled it is the exact result (state 2: hcCnt 2, infoFromHits = the return value).
@@ -3808,8 +3816,8 @@ T4_D inline T4Ovl t4_settle_overlap( T4Ctx &cx, int len, T4Contig *seq, double f
 	}
 	else
 	{
-		int L = t4_min( o.readStart, o.seqStart ) ;
-		int R = t4_min( len - 1 - o.readEnd, seq->len - 1 - o.seqEnd ) ;
+		int L = t4_overhang_side( o, 0, len, seq->len ).n ;
+		int R = t4_overhang_side( o, 1, len, seq->len ).n ;
 		int M = ls.x + rs.x ;
 		int thr = 2 + ( L >= 2 ? 1 : 0 ) + ( R >= 2 ? 1 : 0 ) ;
 		thr = (int)( thr * factor ) ;
@@ -3880,7 +3888,7 @@ T4_D inline void c_overhang_settle( T4Ctx &cx, const T4Ovl *overlaps, int overla
 		T4SideStats ss[2] ;
 		for ( int right = 0 ; right < 2 ; ++right )
 		{
-			int n = right ? t4_min( len - 1 - o.readEnd, seq->len - 1 - o.seqEnd ) : t4_min( o.readStart, o.seqStart ) ;
+			int n = t4_overhang_side( o, right, len, seq->len ).n ;
 			const u32 *bb = bits + 32 * i + 16 * right ;
 			int matches = 0 ;
 			for ( int w = 0 ; w * 32 < n ; ++w )
@@ -3907,8 +3915,749 @@ T4_D inline void c_overhang_settle( T4Ctx &cx, const T4Ovl *overlaps, int overla
 }
 
 // ---------------------------------------------------------------------------
-// SeqSet::AddRead (SeqSet.hpp:3426-4473), novel-contig set.  Collective; reads cx.sm->read / rc.
+// ExtendOverlap of every overlap of a read: the one pass of AddRead and AssignRead
 // ---------------------------------------------------------------------------
+
+// ExtendOverlap (SeqSet.hpp:1165-1277) of every overlap into pre[i]: hcCnt 2 (exact) and infoFromHits = the return
+// value, or one of t4_settle_overlap's lazy states.  Collective; r is the read in the strand of the overlaps.  The
+// masks and side statistics of every overlap come from c_overhang_settle; the sides that need the banded DP are then
+// aligned in one parallel pass (c_overhang_dps), all of them except, when the read is easy, those of a provably-0
+// overlap (state 1).  A read is easy when pre[0] is exact, extends, covers the whole read and is at least
+// easySimilarity similar: a caller that then consults the other overlaps only through their return value may leave
+// them so.  No similarity exceeds 1, so an easySimilarity above 1 makes every overlap exact.
+// Borrows st->failOff for the side statistics and the list of sides to align; the masks stay in st->bitsOff, where
+// s_make_exact reads them.  Returns whether the read is easy.  clk (may be 0): thread 0's clock64() after the settle
+// pass and after the list (device only).
+T4_D inline bool c_extend_overlaps( T4Ctx &cx, const T4Ovl *overlaps, int overlapCnt, const char *r, int len, double factor,
+	double easySimilarity, T4Ovl *pre, long long *clk )
+{
+	T4Stream *st = cx.st ;
+	T4Smem *sm = cx.sm ;
+	if ( cx.tid == 0 )
+		t4_count( cx, 16, (u64)overlapCnt ) ;
+	u32 *bits = cx.P<u32>( st->bitsOff ) ;
+	T4SideStats *sstats = (T4SideStats *)cx.P<char>( st->failOff ) ; // 2 per overlap
+	c_overhang_settle( cx, overlaps, overlapCnt, r, len, factor, bits, sstats, pre ) ;
+#if T4_CUDA
+	if ( clk && cx.tid == 0 )
+		clk[0] = clock64() ;
+#endif
+	bool easy = ( pre[0].hcCnt == 2 && pre[0].infoFromHits == 1 && pre[0].similarity >= easySimilarity
+		&& pre[0].readStart == 0 && pre[0].readEnd == len - 1 ) ;
+	int *pend = (int *)( sstats + 2 * overlapCnt ) ; // the sides to align, in side order (failOff holds a T4Ovl per overlap)
+#if T4_CUDA
+	if ( cx.tid < 32 )
+	{
+		int cnt = 0 ;
+		for ( int base = 0 ; base < 2 * overlapCnt ; base += 32 )
+		{
+			int x = base + cx.tid ;
+			bool p = x < 2 * overlapCnt && sstats[x].ind == -1 && !( easy && pre[x >> 1].hcCnt == 1 ) ;
+			unsigned m = __ballot_sync( T4_FULL, p ) ;
+			if ( p )
+				pend[cnt + __popc( m & ( ( 1u << cx.tid ) - 1u ) )] = x ;
+			cnt += __popc( m ) ;
+		}
+		if ( cx.tid == 0 )
+			sm->bi[0] = cnt ;
+	}
+#else
+	{
+		int cnt = 0 ;
+		for ( int x = 0 ; x < 2 * overlapCnt ; ++x )
+			if ( sstats[x].ind == -1 && !( easy && pre[x >> 1].hcCnt == 1 ) )
+				pend[cnt++] = x ;
+		sm->bi[0] = cnt ;
+	}
+#endif
+	T4_SYNC() ;
+#if T4_CUDA
+	if ( clk && cx.tid == 0 )
+		clk[1] = clock64() ;
+#endif
+	c_overhang_dps( cx, overlaps, r, len, bits, pend, sm->bi[0], sstats ) ;
+	T4_PAR_FOR( i, overlapCnt )
+	{
+		if ( pre[i].hcCnt == 2 || sstats[2 * i].ind == -1 || sstats[2 * i + 1].ind == -1 )
+			continue ;
+		T4Ovl e ;
+		int ok = t4_extend_finish( cx, len, t4_seq( cx, overlaps[i].seqIdx ), factor, overlaps[i], e, sstats[2 * i], sstats[2 * i + 1] ) ;
+		e.infoFromHits = ok ;
+		e.hcCnt = 2 ;
+		pre[i] = e ;
+	}
+	T4_SYNC() ;
+	return easy ;
+}
+
+// ---------------------------------------------------------------------------
+// SeqSet::AddRead (SeqSet.hpp:3426-4473), novel-contig set, in its phases.  c_add_read calls them in order; the
+// decision and the merge hand the collective phases their result in cx.sm->plan.
+// ---------------------------------------------------------------------------
+
+// Gene-name prefix filter (SeqSet.hpp:3445-3472): keeps, in order, the overlaps whose contig name does not start with
+// a capital letter, starts with the first three letters of geneName, or is "Novel".  Collective; the walk is thread
+// 0's.  Returns the new overlap count.
+T4_D inline int c_gene_filter( T4Ctx &cx, T4Ovl *overlaps, int overlapCnt, const char *geneName )
+{
+	T4Smem *sm = cx.sm ;
+	if ( cx.tid == 0 )
+	{
+		int k = 0 ;
+		for ( int i = 0 ; i < overlapCnt ; ++i )
+		{
+			T4Contig *c = t4_seq( cx, overlaps[i].seqIdx ) ;
+			const char *nm = cx.P<char>( c->nameOff ) ;
+			int j = 3 ;
+			if ( nm[0] >= 'A' && nm[0] <= 'Z' )
+			{
+				for ( j = 0 ; j < 3 ; ++j )
+					if ( nm[j] != geneName[j] )
+						break ;
+			}
+			if ( j == 3 || t4_name_eq( nm, c->nameLen, "Novel", 5 ) )
+			{
+				if ( k != i )
+					overlaps[k] = overlaps[i] ;
+				++k ;
+			}
+		}
+		sm->bi[0] = k ;
+	}
+	T4_SYNC() ;
+	overlapCnt = sm->bi[0] ;
+	T4_SYNC() ;
+	return overlapCnt ;
+}
+
+// The decision walk (SeqSet.hpp:3476-3877): from the sorted overlaps and their ExtendOverlap results pre[] to the
+// extended overlaps to commit, extendedOverlaps[0 .. k), updating the contigs' extension anchors on the way.  Makes an
+// overlap exact on demand (s_make_exact) where pre[] holds no exact result.  Thread 0.  Borrows st->failOff for the
+// failed extended overlaps and st->anchorOff for the old anchors.  Returns k; sortExtendedOverlaps: whether the merge
+// sorts the extended overlaps by read start.
+T4_D inline int s_decide_overlaps( T4Ctx &cx, const T4Ovl *overlaps, int overlapCnt, const char *r, int len, double factor, T4Ovl *pre,
+	int minKmerCount, double similarityThreshold, T4Ovl *extendedOverlaps, bool &sortExtendedOverlaps )
+{
+	T4Stream *st = cx.st ;
+	T4Ovl *failedExtendedOverlaps = cx.P<T4Ovl>( st->failOff ) ;
+	int *oldMinExtAnchor = cx.P<int>( st->anchorOff ) ;
+	const int radius = st->radius ;
+	int i, j, k = 0 ;
+	int failedExtendedOverlapsCnt = 0 ;
+	T4Ovl goodExtendedOverlap ;
+	goodExtendedOverlap.seqIdx = -1 ;
+	int tag = 0 ;
+	sortExtendedOverlaps = true ;
+
+	for ( i = 0 ; i < overlapCnt ; ++i )
+	{
+		T4Contig *seq = t4_seq( cx, overlaps[i].seqIdx ) ;
+		oldMinExtAnchor[2 * i] = seq->minLeftExtAnchor ;
+		oldMinExtAnchor[2 * i + 1] = seq->minRightExtAnchor ;
+		for ( j = 0 ; j < k ; ++j )
+		{
+			int leftRadius = radius, rightRadius = radius ;
+			if ( extendedOverlaps[j].seqStart == 0 )
+				leftRadius = 0 ;
+			if ( extendedOverlaps[j].seqEnd == t4_seq( cx, extendedOverlaps[j].seqIdx )->len - 1 )
+				rightRadius = 0 ;
+			if ( overlaps[i].readStart >= extendedOverlaps[j].readStart - leftRadius
+				&& overlaps[i].readEnd <= extendedOverlaps[j].readEnd + rightRadius
+				&& ( overlaps[i].seqStart >= radius || overlaps[i].seqEnd <= seq->len - radius - 1 ) )
+				break ;
+			leftRadius = radius ;
+			rightRadius = radius ;
+			if ( overlaps[i].seqStart == 0 )
+				leftRadius = 0 ;
+			if ( overlaps[i].seqEnd == seq->len - 1 )
+				rightRadius = 0 ;
+			if ( extendedOverlaps[j].readStart >= overlaps[i].readStart - leftRadius
+				&& extendedOverlaps[j].readEnd <= overlaps[i].readEnd + rightRadius )
+				break ;
+		}
+		if ( j < k )
+			continue ;
+		if ( pre[i].hcCnt != 2 )
+			s_make_exact( cx, r, len, factor, overlaps, pre, i ) ;
+		extendedOverlaps[k] = pre[i] ;
+		if ( pre[i].infoFromHits == 1 )
+		{
+			T4Ovl &eo = extendedOverlaps[k] ;
+			if ( eo.similarity < similarityThreshold )
+			{
+				if ( ( minKmerCount <= 1 || eo.similarity + 0.01 >= similarityThreshold ) && eo.readStart == 0
+					&& eo.readEnd == len - 1 )
+					goodExtendedOverlap = eo ;
+				continue ;
+			}
+			for ( j = 0 ; j < k ; ++j )
+			{
+				int leftRadius = radius, rightRadius = radius ;
+				if ( extendedOverlaps[j].seqStart == 0 )
+					leftRadius = 0 ;
+				if ( extendedOverlaps[j].seqEnd == t4_seq( cx, extendedOverlaps[j].seqIdx )->len - 1 )
+					rightRadius = 0 ;
+				if ( eo.readStart >= extendedOverlaps[j].readStart - leftRadius
+					&& eo.readEnd <= extendedOverlaps[j].readEnd + rightRadius
+					&& ( overlaps[i].seqStart > 0 || overlaps[i].seqEnd < seq->len - 1 ) )
+					break ;
+				if ( extendedOverlaps[j].readStart >= eo.readStart - radius && extendedOverlaps[j].readEnd <= eo.readEnd + radius )
+					break ;
+			}
+			if ( j < k )
+				continue ;
+			T4Contig *eseq = t4_seq( cx, eo.seqIdx ) ;
+			int span = eo.readEnd - eo.readStart + 1 ;
+			for ( j = 0 ; j < i ; ++j )
+			{
+				if ( eo.seqStart == 0 && eo.seqEnd == eseq->len - 1 )
+					continue ;
+				if ( eo.readStart >= overlaps[j].readStart && eo.readEnd <= overlaps[j].readEnd
+					&& ( overlaps[j].readEnd - overlaps[j].readStart >= eo.readEnd - eo.readStart + 10
+						|| overlaps[j].similarity + 0.02 >= eo.similarity ) )
+				{
+					if ( eo.readStart > 0 && eseq->minLeftExtAnchor < span )
+						eseq->minLeftExtAnchor = span ;
+					if ( eo.readEnd < len - 1 && eseq->minRightExtAnchor < span )
+						eseq->minRightExtAnchor = span ;
+					break ;
+				}
+			}
+			if ( j < i )
+				continue ;
+			for ( j = 0 ; j < failedExtendedOverlapsCnt ; ++j )
+			{
+				if ( eo.seqStart == 0 && eo.seqEnd == eseq->len - 1 )
+					continue ;
+				if ( eo.readStart >= failedExtendedOverlaps[j].readStart && eo.readEnd <= failedExtendedOverlaps[j].readEnd )
+				{
+					if ( eo.readStart > 0 && eseq->minLeftExtAnchor < span )
+						eseq->minLeftExtAnchor = span ;
+					if ( eo.readEnd < len - 1 && eseq->minRightExtAnchor < span )
+						eseq->minRightExtAnchor = span ;
+					break ;
+				}
+			}
+			if ( j < failedExtendedOverlapsCnt )
+				continue ;
+			if ( eo.readStart > 0 && eseq->minLeftExtAnchor >= span )
+				continue ;
+			if ( eo.readEnd < len - 1 && eseq->minRightExtAnchor >= span )
+				continue ;
+			tag = i ;
+			++k ;
+		}
+		else
+		{
+			failedExtendedOverlaps[failedExtendedOverlapsCnt] = extendedOverlaps[k] ;
+			++failedExtendedOverlapsCnt ;
+		}
+	}
+
+	if ( k == 1 && extendedOverlaps[0].readStart <= radius && extendedOverlaps[0].readEnd >= len - radius )
+	{
+		// could the read bridge to a second contig? (SeqSet.hpp:3732-3793)
+		for ( i = 0 ; i < overlapCnt ; ++i )
+		{
+			if ( tag == i )
+				continue ;
+			if ( pre[i].hcCnt == 1 )
+				continue ; // ExtendOverlap provably returns 0; only the return value is consulted here
+			if ( pre[i].hcCnt != 2 )
+				s_make_exact( cx, r, len, factor, overlaps, pre, i ) ;
+			extendedOverlaps[k] = pre[i] ;
+			if ( pre[i].infoFromHits == 1 )
+			{
+				j = i ;
+				++k ;
+			}
+		}
+		if ( k > 2 )
+			k = 1 ;
+		else if ( k == 2 )
+		{
+			int span = extendedOverlaps[1].readEnd - extendedOverlaps[1].readStart + 1 ;
+			if ( extendedOverlaps[1].readStart > 0 && oldMinExtAnchor[2 * j] >= span )
+				k = 1 ;
+			if ( extendedOverlaps[1].readEnd < len - 1 && oldMinExtAnchor[2 * j + 1] >= span )
+				k = 1 ;
+			if ( k == 2 )
+			{
+				if ( extendedOverlaps[0].seqEnd == t4_seq( cx, extendedOverlaps[0].seqIdx )->len - 1
+					&& extendedOverlaps[1].seqStart == 0 )
+					sortExtendedOverlaps = false ;
+				else if ( extendedOverlaps[0].seqStart == 0
+					&& extendedOverlaps[1].seqEnd == t4_seq( cx, extendedOverlaps[1].seqIdx )->len - 1 )
+				{
+					sortExtendedOverlaps = false ;
+					T4Ovl tmp = extendedOverlaps[0] ;
+					extendedOverlaps[0] = extendedOverlaps[1] ;
+					extendedOverlaps[1] = tmp ;
+				}
+				else
+					k = 1 ;
+			}
+		}
+	}
+
+	if ( similarityThreshold > st->novelSeqSimilarity )
+	{
+		int cnt = 0 ;
+		for ( i = 0 ; i < k ; ++i )
+			if ( extendedOverlaps[i].similarity >= similarityThreshold )
+			{
+				extendedOverlaps[cnt] = extendedOverlaps[i] ;
+				++cnt ;
+			}
+		k = cnt ;
+	}
+	if ( k == 0 && goodExtendedOverlap.seqIdx != -1 )
+	{
+		extendedOverlaps[0] = goodExtendedOverlap ;
+		k = 1 ;
+	}
+	if ( k > 1 )
+	{
+		for ( i = 0 ; i < k ; ++i )
+			if ( extendedOverlaps[i].similarity >= 0.95 )
+				break ;
+		if ( i >= k )
+		{
+			int maxtag = 0 ;
+			for ( i = 1 ; i < k ; ++i )
+				if ( t4_ovl_less( extendedOverlaps[i], extendedOverlaps[maxtag] ) )
+					maxtag = i ;
+			extendedOverlaps[0] = extendedOverlaps[maxtag] ;
+			k = 1 ;
+		}
+	}
+	if ( k > 1 )
+	{
+		for ( i = 0 ; i < k - 1 ; ++i )
+			for ( j = i + 1 ; j < k ; ++j )
+				if ( extendedOverlaps[i].seqIdx == extendedOverlaps[j].seqIdx )
+				{
+					k = 0 ;
+					break ;
+				}
+	}
+	return k ;
+}
+
+// The merge commit (SeqSet.hpp:3878-4130) of the k > 1 extended overlaps extendedOverlaps[0 .. k): one contig from all
+// of them and the read.  Rare (0.7 % of AddReads).  Thread 0.  Writes plan's kind, added, bail, ret, seqIdx and
+// readInConsensusOffset.  Borrows seqOffset (st->extOff, whose pre[] is dead after the decision) for the contigs'
+// positions in the merged contig.
+T4_D inline void s_merge_commit( T4Ctx &cx, T4Ovl *extendedOverlaps, int k, bool sortExtendedOverlaps, const char *r, int len,
+	int barcode, int *seqOffset, T4AddPlan &plan )
+{
+	int i, j ;
+	int eOverlapCnt = k ;
+	plan.added = true ;
+	plan.kind = 2 ;
+	if ( sortExtendedOverlaps )
+	{
+		// std::sort by readStart only; equal keys would make the order implementation defined, so keep the
+		// sort stable and flag ties (they need differing contigs with equal extended read starts)
+		for ( i = 1 ; i < eOverlapCnt ; ++i )
+		{
+			T4Ovl x = extendedOverlaps[i] ;
+			for ( j = i - 1 ; j >= 0 && extendedOverlaps[j].readStart > x.readStart ; --j )
+				extendedOverlaps[j + 1] = extendedOverlaps[j] ;
+			extendedOverlaps[j + 1] = x ;
+		}
+	}
+	for ( i = 0 ; i < k && !plan.bail ; ++i )
+		for ( j = i + 1 ; j < k ; ++j )
+		{
+			T4Contig *ca = t4_seq( cx, extendedOverlaps[i].seqIdx ) ;
+			T4Contig *cb = t4_seq( cx, extendedOverlaps[j].seqIdx ) ;
+			if ( !t4_name_compatible( cx.P<char>( ca->nameOff ), ca->nameLen, cx.P<char>( cb->nameOff ), cb->nameLen ) )
+			{
+				plan.bail = true ;
+				break ;
+			}
+		}
+	if ( plan.bail )
+		plan.ret = -1 ;
+	else
+	{
+		int sum = 0 ;
+		for ( i = 0 ; i < eOverlapCnt ; ++i )
+			sum += t4_seq( cx, extendedOverlaps[i].seqIdx )->len ;
+		// positions of the contigs in the merged contig
+		if ( extendedOverlaps[0].readStart > 0 )
+		{
+			for ( i = 0 ; i < eOverlapCnt ; ++i )
+				seqOffset[i] = extendedOverlaps[i].readStart ;
+		}
+		else
+		{
+			seqOffset[0] = 0 ;
+			for ( i = 1 ; i < eOverlapCnt ; ++i )
+				seqOffset[i] = seqOffset[i - 1] + t4_seq( cx, extendedOverlaps[i - 1].seqIdx )->len - 1
+					+ ( extendedOverlaps[i].readStart - extendedOverlaps[i - 1].readEnd ) ;
+		}
+		u64 ncOff = s_alloc( cx, (u64)( sum + len + 1 ) + 16 ) ;
+		if ( ncOff )
+		{
+			char *newConsensus = cx.P<char>( ncOff ) ;
+			if ( extendedOverlaps[0].readStart > 0 )
+				memcpy( newConsensus, r, len ) ;
+			else
+				memcpy( newConsensus + extendedOverlaps[0].seqStart, r, len ) ;
+			for ( i = eOverlapCnt - 1 ; i >= 0 ; --i )
+			{
+				T4Contig *c = t4_seq( cx, extendedOverlaps[i].seqIdx ) ;
+				memcpy( newConsensus + seqOffset[i], t4_cons( cx, c ), c->len ) ;
+			}
+			int newConsensusLen = 0 ;
+			int lastEndExtendedOverlapIdx = eOverlapCnt - 1 ;
+			k = 0 ;
+			for ( i = 0 ; i < eOverlapCnt ; ++i )
+			{
+				int e = seqOffset[i] + t4_seq( cx, extendedOverlaps[i].seqIdx )->len ;
+				if ( e > k )
+				{
+					k = e ;
+					lastEndExtendedOverlapIdx = i ;
+				}
+			}
+			if ( extendedOverlaps[lastEndExtendedOverlapIdx].readEnd < len )
+				newConsensusLen = k + ( len - extendedOverlaps[lastEndExtendedOverlapIdx].readEnd - 1 ) ;
+			else
+				newConsensusLen = k ;
+
+			int newSeqIdx = extendedOverlaps[0].seqIdx ;
+			k = 0 ;
+			for ( i = 1 ; i < eOverlapCnt ; ++i )
+				if ( extendedOverlaps[i].seqIdx < newSeqIdx )
+				{
+					newSeqIdx = extendedOverlaps[i].seqIdx ;
+					k = i ;
+				}
+			// index removal uses the OLD consensus of every participant
+			for ( i = 0 ; i < eOverlapCnt ; ++i )
+			{
+				T4Contig *c = t4_seq( cx, extendedOverlaps[i].seqIdx ) ;
+				s_remove_index( cx, t4_cons( cx, c ), c->len, extendedOverlaps[i].seqIdx, barcode, 0 ) ;
+			}
+			// new posWeight: old columns of newSeqIdx shifted by seqOffset[k], zero elsewhere, plus the others
+			T4Contig *ns = t4_seq( cx, newSeqIdx ) ;
+			int oldLen = ns->len ;
+			int cap = 2 * newConsensusLen + 128 ;
+			u64 co = s_alloc( cx, cap ) ;
+			u64 po = s_alloc( cx, T4_PW_BYTES( cap ) ) ;
+			if ( co && po )
+			{
+				int lead = ( cap - newConsensusLen ) / 2 ;
+				int *npw = cx.P<int>( po ) + 4 * lead ;
+				unsigned char *neq = cx.P<unsigned char>( po + 16ull * cap ) + lead ;
+				int *opw = t4_pw( cx, ns ) ;
+				for ( i = 0 ; i < 4 * newConsensusLen ; ++i )
+					npw[i] = 0 ;
+				for ( i = 0 ; i < 4 * oldLen ; ++i )
+					npw[4 * seqOffset[k] + i] = opw[i] ;
+				for ( i = 0 ; i < eOverlapCnt ; ++i )
+				{
+					int sIdx = extendedOverlaps[i].seqIdx ;
+					if ( sIdx == newSeqIdx )
+						continue ;
+					T4Contig *c = t4_seq( cx, sIdx ) ;
+					ns->numRead += c->numRead ;
+					int *cpw = t4_pw( cx, c ) ;
+					for ( j = 0 ; j < 4 * c->len ; ++j )
+						npw[4 * seqOffset[i] + j] += cpw[j] ;
+				}
+				for ( i = 0 ; i < newConsensusLen ; ++i )
+					neq[i] = (unsigned char)t4_eq_nibble( npw + 4 * i ) ;
+				// name (SeqSet.hpp:4066-4096)
+				int nameIdx ;
+				for ( nameIdx = 0 ; nameIdx < eOverlapCnt ; ++nameIdx )
+				{
+					T4Contig *c = t4_seq( cx, extendedOverlaps[nameIdx].seqIdx ) ;
+					if ( !t4_name_eq( cx.P<char>( c->nameOff ), c->nameLen, "Novel", 5 ) )
+						break ;
+				}
+				if ( nameIdx >= eOverlapCnt )
+					nameIdx = 0 ;
+				int nameSum = 0 ;
+				for ( i = 0 ; i < eOverlapCnt ; ++i )
+					nameSum += t4_seq( cx, extendedOverlaps[i].seqIdx )->nameLen ;
+				u64 nbOff = s_alloc( cx, nameSum + eOverlapCnt + 1 ) ;
+				if ( nbOff )
+				{
+					char *nameBuffer = cx.P<char>( nbOff ) ;
+					T4Contig *c0 = t4_seq( cx, extendedOverlaps[nameIdx].seqIdx ) ;
+					memcpy( nameBuffer, cx.P<char>( c0->nameOff ), c0->nameLen ) ;
+					int nl = c0->nameLen ;
+					for ( i = 0 ; i < eOverlapCnt ; ++i )
+					{
+						if ( i == nameIdx )
+							continue ;
+						if ( i > 0 )
+						{
+							T4Contig *ci = t4_seq( cx, extendedOverlaps[i].seqIdx ) ;
+							T4Contig *cp = t4_seq( cx, extendedOverlaps[i - 1].seqIdx ) ;
+							if ( !t4_name_eq( cx.P<char>( ci->nameOff ), ci->nameLen, cx.P<char>( cp->nameOff ), cp->nameLen ) )
+							{
+								nameBuffer[nl] = '+' ;
+								memcpy( nameBuffer + nl + 1, cx.P<char>( ci->nameOff ), ci->nameLen ) ;
+								nl += 1 + ci->nameLen ;
+							}
+						}
+					}
+					nameBuffer[nl] = '\0' ;
+					int minLeft = t4_seq( cx, extendedOverlaps[0].seqIdx )->minLeftExtAnchor ;
+					int minRight = t4_seq( cx, extendedOverlaps[lastEndExtendedOverlapIdx].seqIdx )->minRightExtAnchor ;
+					// release the merged-away contigs (SeqSet::ReleaseSeq: the slot stays, NULL consensus)
+					for ( i = 0 ; i < eOverlapCnt ; ++i )
+					{
+						int sIdx = extendedOverlaps[i].seqIdx ;
+						if ( sIdx == newSeqIdx )
+							continue ;
+						T4Contig *c = t4_seq( cx, sIdx ) ;
+						c->consOff = 0 ;
+						c->pwOff = 0 ;
+						c->nameOff = 0 ;
+						c->len = 0 ;
+					}
+					ns->nameOff = nbOff ;
+					ns->nameLen = nl ;
+					ns->consOff = co ;
+					ns->pwOff = po ;
+					ns->cap = cap ;
+					ns->lead = lead ;
+					ns->len = newConsensusLen ;
+					memcpy( t4_cons( cx, ns ), newConsensus, newConsensusLen ) ;
+					s_update_consensus( cx, newSeqIdx, false ) ;
+					s_build_index( cx, t4_cons( cx, ns ), newConsensusLen, newSeqIdx, barcode, 0 ) ;
+					ns->minLeftExtAnchor = minLeft ;
+					ns->minRightExtAnchor = minRight ;
+					plan.readInConsensusOffset = 0 ;
+					if ( extendedOverlaps[0].seqStart > 0 )
+						plan.readInConsensusOffset = extendedOverlaps[0].seqStart ;
+					plan.seqIdx = newSeqIdx ;
+				}
+			}
+		}
+	}
+}
+
+// The extend / inside commit (SeqSet.hpp:4131-4316) of the one extended overlap p.e0: grows its contig by the read's
+// overhangs (index first, in the reference's order), decays the end weights and applies the scheduled consensus
+// substitutions.  Collective.  Sets p.seqIdx and p.readInConsensusOffset, or p.ret and p.bail when the contig cannot
+// grow.  Borrows tmpc (st->extOff, whose pre[] is dead after the decision) for the new left k-mers, and sm->bi[0 .. 9]
+// for broadcasts within the phase.
+T4_D inline void c_extend_commit( T4Ctx &cx, T4AddPlan &p, const char *r, int len, int barcode, int minKmerCount, char *tmpc )
+{
+	T4Stream *st = cx.st ;
+	T4Smem *sm = cx.sm ;
+	const T4Ovl &e0 = p.e0 ;
+	const int seqIdx = e0.seqIdx ;
+	p.seqIdx = seqIdx ;
+	T4Contig *seq = t4_seq( cx, seqIdx ) ;
+	if ( cx.tid == 0 )
+		++seq->numRead ;
+	if ( e0.readStart > 0 || e0.readEnd < len - 1 )
+	{
+		const int shift = e0.readStart ;
+		const int rightAdd = ( e0.readEnd < len - 1 ) ? ( len - 1 - e0.readEnd ) : 0 ;
+		const int oldLen = seq->len ;
+		const int kl = st->kmerLength ;
+		// index first, in the reference's order: new left k-mers, shift the old postings, (later) new right k-mers
+		if ( shift > 0 )
+		{
+			char *oldCons = t4_cons( cx, seq ) ;
+			// tmpc: newConsensus[0 .. shift + kl - 1): read prefix + the first kl-1 old bases
+			int n = shift + kl - 1 ;
+			T4_PAR_FOR( i, n )
+			{
+				char c ;
+				if ( i < shift )
+					c = r[i] ;
+				else if ( i - shift < oldLen )
+					c = oldCons[i - shift] ;
+				else
+				{
+					int ri = e0.readEnd + 1 + ( i - shift - oldLen ) ;
+					c = ( ri < len ) ? r[ri] : '\0' ;
+				}
+				tmpc[i] = c ;
+			}
+			T4_SYNC() ;
+			c_index_op( cx, tmpc, n, T4_IDX_BUILD, seqIdx, barcode, 0, 0 ) ;
+			c_index_op( cx, oldCons, oldLen, T4_IDX_UPDATE, seqIdx, barcode, shift, seqIdx ) ;
+		}
+		T4_SYNC() ; // every thread has read the old length / pointers
+		if ( cx.tid == 0 )
+			sm->bi[0] = s_contig_grow( cx, seq, shift, rightAdd ) ? 1 : 0 ;
+		T4_SYNC() ;
+		bool grown = sm->bi[0] != 0 ;
+		T4_SYNC() ;
+		if ( !grown )
+		{
+			p.ret = T4_E_NOMEM ;
+			p.bail = true ;
+		}
+		else
+		{
+			char *newConsensus = t4_cons( cx, seq ) ;
+			int *pw = t4_pw( cx, seq ) ;
+			unsigned char *eq = t4_eq( cx, seq ) ;
+			const int newConsensusLen = seq->len ;
+			T4_PAR_FOR( i, shift )
+				newConsensus[i] = r[i] ;
+			T4_PAR_FOR( x, rightAdd )
+				newConsensus[shift + oldLen + x] = r[e0.readEnd + 1 + x] ;
+			T4_PAR_FOR( i, shift )
+				t4_col_put( pw, eq, i, 0, 0, 0, 0 ) ;
+			T4_PAR_FOR( i, rightAdd )
+				t4_col_put( pw, eq, shift + oldLen + i, 0, 0, 0, 0 ) ;
+			T4_SYNC() ;
+			if ( e0.readEnd < len - 1 )
+			{
+				int start = e0.readStart + e0.seqEnd - kl + 2 ;
+				if ( start < 0 )
+				{
+					if ( cx.tid == 0 )
+						t4_raise( cx, T4_E_INTERNAL, 11 ) ;
+					start = 0 ;
+				}
+				c_index_op( cx, newConsensus + start, newConsensusLen - start, T4_IDX_BUILD, seqIdx, barcode, start, 0 ) ;
+			}
+			// end-weight decay and scheduled consensus substitutions (SeqSet.hpp:4192-4247): four columns, serial
+			if ( cx.tid == 0 )
+			{
+				int nrep = 0 ;
+				if ( shift > 0 && ( barcode == -1 || minKmerCount > 1 ) )
+				{
+					for ( int i = 0 ; i < 2 ; ++i )
+					{
+						if ( i + shift >= len || r[i + shift] == 'N' )
+							continue ;
+						char nc = newConsensus[i + shift] ;
+						if ( r[i + shift] != nc && nc != 'N' && pw[4 * ( i + shift ) + t4_nuc( nc )] == 1 )
+						{
+							sm->bi[2 + nrep] = i + shift ;
+							sm->bi[6 + nrep] = r[i + shift] ;
+							++nrep ;
+						}
+						for ( int j = 0 ; j < 4 ; ++j )
+							if ( r[i + shift] != t4_numToNuc( j ) && pw[4 * ( i + shift ) + j] > 1 )
+								t4_col_add( pw, eq, i + shift, j, -1 ) ;
+					}
+				}
+				if ( e0.readEnd < len - 1 && ( barcode == -1 || minKmerCount > 1 ) )
+				{
+					for ( int i = oldLen - 2 ; i < oldLen ; ++i )
+					{
+						int pos = i - e0.seqStart ;
+						int seqPos = i + shift ;
+						if ( pos < 0 || r[pos] == 'N' )
+							continue ;
+						if ( i < 0 )
+						{
+							t4_raise( cx, T4_E_INTERNAL, 12 ) ;
+							continue ;
+						}
+						char nc = newConsensus[seqPos] ;
+						if ( r[pos] != nc && nc != 'N' && pw[4 * seqPos + t4_nuc( nc )] == 1 )
+						{
+							sm->bi[2 + nrep] = seqPos ;
+							sm->bi[6 + nrep] = r[pos] ;
+							++nrep ;
+						}
+						for ( int j = 0 ; j < 4 ; ++j )
+							if ( r[pos] != t4_numToNuc( j ) && pw[4 * seqPos + j] > 1 )
+								t4_col_add( pw, eq, seqPos, j, -1 ) ;
+					}
+				}
+				if ( shift > 0 )
+					seq->minLeftExtAnchor = 0 ;
+				if ( e0.readEnd < len - 1 )
+					seq->minRightExtAnchor = 0 ;
+				sm->bi[1] = nrep ;
+			}
+			T4_SYNC() ;
+			// (the +GENE name adjustment needs isRef overlaps: never in the stage-1 novel set, SeqSet.hpp:4258-4296)
+			p.readInConsensusOffset = 0 ;
+			if ( e0.seqStart > 0 )
+				p.readInConsensusOffset = e0.seqStart ;
+			int nrep = sm->bi[1] ;
+			int repPos[4], repChar[4] ;
+			for ( int i = 0 ; i < nrep ; ++i )
+			{
+				repPos[i] = sm->bi[2 + i] ;
+				repChar[i] = sm->bi[6 + i] ;
+			}
+			T4_SYNC() ;
+			for ( int i = 0 ; i < nrep ; ++i )
+				c_substitute_consensus_pos( cx, seqIdx, repPos[i], (char)repChar[i] ) ;
+		}
+	}
+	else
+		p.readInConsensusOffset = e0.seqStart ;
+}
+
+// The posWeight update (SeqSet.hpp:4318-4363): adds the read to the columns of contig seqIdx from
+// readInConsensusOffset on, then fills the consensus N's under the read and indexes their k-mers (thread 0; rare).
+// Collective.  strand: the overlaps' strand.  Borrows nPos (st->extOff, whose pre[] is dead after the decision) for
+// the read positions of those N's, and sm->bi[0] within the phase.
+T4_D inline void c_posweight_update( T4Ctx &cx, int seqIdx, int readInConsensusOffset, const char *r, int len, int barcode, int strand,
+	int *nPos )
+{
+	T4Stream *st = cx.st ;
+	T4Smem *sm = cx.sm ;
+	T4Contig *seq = t4_seq( cx, seqIdx ) ;
+	char *cons = t4_cons( cx, seq ) ;
+	int *pw = t4_pw( cx, seq ) ;
+	unsigned char *eq = t4_eq( cx, seq ) ;
+	if ( cx.tid == 0 )
+		sm->bi[0] = 0 ;
+	T4_SYNC() ;
+	T4_PAR_FOR( i, len )
+	{
+		if ( r[i] == 'N' )
+			continue ;
+		t4_col_add( pw, eq, i + readInConsensusOffset, t4_nuc( r[i] ), 1 ) ;
+		if ( cons[i + readInConsensusOffset] == 'N' )
+			sm->bi[0] = 1 ;
+	}
+	T4_SYNC() ;
+	if ( cx.tid == 0 )
+	{
+		t4_set_prev( st, seqIdx, 0, len - 1, readInConsensusOffset, strand ) ;
+		if ( sm->bi[0] )
+		{
+			// consensus N's under the read are filled and their k-mers indexed (SeqSet.hpp:4338-4360); rare
+			int kl = st->kmerLength ;
+			int size = 0 ;
+			for ( int i = 0 ; i < len ; ++i )
+				if ( r[i] != 'N' && cons[i + readInConsensusOffset] == 'N' )
+					nPos[size++] = i ;
+			for ( int i = 0 ; i < size ; )
+			{
+				int j ;
+				for ( j = i + 1 ; j < size ; ++j )
+					if ( nPos[j] > nPos[j - 1] + kl - 1 )
+						break ;
+				for ( int l = i ; l < j ; ++l )
+					cons[nPos[l] + readInConsensusOffset] = r[nPos[l]] ;
+				int start = nPos[i] - kl + 1 + readInConsensusOffset ;
+				if ( start < 0 )
+					start = 0 ;
+				int end = nPos[j - 1] + kl - 1 + readInConsensusOffset ;
+				if ( end >= seq->len )
+					end = seq->len - 1 ;
+				s_build_index( cx, cons + start, end - start + 1, seqIdx, barcode, start ) ;
+				i = j ;
+			}
+		}
+	}
+}
+
+// SeqSet::AddRead (SeqSet.hpp:3426-4473), novel-contig set.  Collective; reads cx.sm->read / rc.
 T4_D T4_BIG int c_add_read( T4Ctx &cx, int len, const char *geneName, int &strand, int barcode, int minKmerCount,
 	bool repetitiveData, double similarityThreshold )
 {
@@ -3923,35 +4672,9 @@ T4_D T4_BIG int c_add_read( T4Ctx &cx, int len, const char *geneName, int &stran
 	if ( overlapCnt <= 0 )
 		return -1 ;
 	T4Ovl *overlaps = cx.P<T4Ovl>( st->ovlOff ) ;
-	// gene-name prefix filter (SeqSet.hpp:3445-3472)
 	if ( geneName[0] != '\0' )
 	{
-		if ( cx.tid == 0 )
-		{
-			int k = 0 ;
-			for ( int i = 0 ; i < overlapCnt ; ++i )
-			{
-				T4Contig *c = t4_seq( cx, overlaps[i].seqIdx ) ;
-				const char *nm = cx.P<char>( c->nameOff ) ;
-				int j = 3 ;
-				if ( nm[0] >= 'A' && nm[0] <= 'Z' )
-				{
-					for ( j = 0 ; j < 3 ; ++j )
-						if ( nm[j] != geneName[j] )
-							break ;
-				}
-				if ( j == 3 || t4_name_eq( nm, c->nameLen, "Novel", 5 ) )
-				{
-					if ( k != i )
-						overlaps[k] = overlaps[i] ;
-					++k ;
-				}
-			}
-			sm->bi[0] = k ;
-		}
-		T4_SYNC() ;
-		overlapCnt = sm->bi[0] ;
-		T4_SYNC() ;
+		overlapCnt = c_gene_filter( cx, overlaps, overlapCnt, geneName ) ;
 		if ( overlapCnt <= 0 )
 			return -1 ;
 	}
@@ -3959,730 +4682,71 @@ T4_D T4_BIG int c_add_read( T4Ctx &cx, int len, const char *geneName, int &stran
 
 	const char *r = ( overlaps[0].strand == 1 ) ? sm->read : sm->rc ;
 	const double factor = ( barcode == -1 && !repetitiveData ) ? 1.0 : 2.0 ;
-	// ExtendOverlap is a pure function of (overlap, read, contig): evaluate it for every overlap up front
+	T4Ovl *pre = cx.P<T4Ovl>( st->extOff ) ; // ExtendOverlap of every overlap; scratch of the commits after the decision
 	T4_PHASE( cx, 5 ) ;
+	long long xt[4] = { 0, 0, 0, 0 } ; // thread 0's clock64() around and inside the pass: counters 17-19
+#if T4_CUDA
+	xt[0] = clock64() ;
+#endif
+	const bool easy = c_extend_overlaps( cx, overlaps, overlapCnt, r, len, factor, similarityThreshold, pre, xt + 1 ) ;
+#if T4_CUDA
 	if ( cx.tid == 0 )
-		t4_count( cx, 16, (u64)overlapCnt ) ;
-	T4Ovl *pre = cx.P<T4Ovl>( st->extOff ) ;
 	{
-		{
-		// masks, side statistics and pre[] of every overlap; the DP sides are deferred to c_overhang_dps below, which may
-		// leave an overlap to the decision loop to make exact on demand (s_make_exact)
-#if T4_CUDA
-		long long xt0 = clock64() ;
-#endif
-		u32 *bits = cx.P<u32>( st->bitsOff ) ;
-		T4SideStats *sstats = (T4SideStats *)cx.P<char>( st->failOff ) ; // scratch: 2 per overlap (failOff is unused until the decision)
-		c_overhang_settle( cx, overlaps, overlapCnt, r, len, factor, bits, sstats, pre ) ;
-#if T4_CUDA
-		long long xt1 = clock64() ;
-#endif
-		// Every deferred side the decision loop may consult is aligned now, in one parallel pass, except the sides of a
-		// provably-0 overlap of an easy read (the best overlap is settled, extends, clears the threshold and covers the
-		// whole read).  The decision loop then consults the other overlaps (almost) only through the bridging loop,
-		// where state 1 suffices; the rare overlap it consults without a result is made exact on demand (s_make_exact).
-		bool easy = ( pre[0].hcCnt == 2 && pre[0].infoFromHits == 1 && pre[0].similarity >= similarityThreshold
-			&& pre[0].readStart == 0 && pre[0].readEnd == len - 1 ) ;
-		int *pend = (int *)( sstats + 2 * overlapCnt ) ; // the sides to align, in side order (failOff holds a T4Ovl per overlap)
-#if T4_CUDA
-		if ( cx.tid < 32 )
-		{
-			int cnt = 0 ;
-			for ( int base = 0 ; base < 2 * overlapCnt ; base += 32 )
-			{
-				int x = base + cx.tid ;
-				bool p = x < 2 * overlapCnt && sstats[x].ind == -1 && !( easy && pre[x >> 1].hcCnt == 1 ) ;
-				unsigned m = __ballot_sync( T4_FULL, p ) ;
-				if ( p )
-					pend[cnt + __popc( m & ( ( 1u << cx.tid ) - 1u ) )] = x ;
-				cnt += __popc( m ) ;
-			}
-			if ( cx.tid == 0 )
-				sm->bi[0] = cnt ;
-		}
-#else
-		{
-			int cnt = 0 ;
-			for ( int x = 0 ; x < 2 * overlapCnt ; ++x )
-				if ( sstats[x].ind == -1 && !( easy && pre[x >> 1].hcCnt == 1 ) )
-					pend[cnt++] = x ;
-			sm->bi[0] = cnt ;
-		}
-#endif
-		T4_SYNC() ;
-#if T4_CUDA
-		long long xt2 = clock64() ;
-#endif
-		c_overhang_dps( cx, overlaps, r, len, bits, pend, sm->bi[0], sstats ) ;
-		T4_PAR_FOR( i, overlapCnt )
-		{
-			if ( pre[i].hcCnt == 2 || sstats[2 * i].ind == -1 || sstats[2 * i + 1].ind == -1 )
-				continue ;
-			T4Ovl e ;
-			int ok = t4_extend_finish( cx, len, t4_seq( cx, overlaps[i].seqIdx ), factor, overlaps[i], e, sstats[2 * i], sstats[2 * i + 1] ) ;
-			e.infoFromHits = ok ;
-			e.hcCnt = 2 ;
-			pre[i] = e ;
-		}
-#if T4_CUDA
-		T4_SYNC() ;
-		if ( cx.tid == 0 )
-		{
-			long long xt3 = clock64() ;
-			t4_count( cx, 17, (u64)( xt1 - xt0 ) ) ;
-			t4_count( cx, 18, (u64)( xt2 - xt1 ) ) ;
-			t4_count( cx, 19, (u64)( xt3 - xt2 ) ) ;
-			t4_count( cx, 20, easy ? 1 : 0 ) ;
-		}
-#endif
-		}
+		xt[3] = clock64() ;
+		t4_count( cx, 17, (u64)( xt[1] - xt[0] ) ) ;
+		t4_count( cx, 18, (u64)( xt[2] - xt[1] ) ) ;
+		t4_count( cx, 19, (u64)( xt[3] - xt[2] ) ) ;
+		t4_count( cx, 20, easy ? 1 : 0 ) ;
 	}
-	T4_SYNC() ;
+#else
+	(void)easy ;
+#endif
 	T4_PHASE( cx, 6 ) ;
 	if ( cx.tid == 0 )
 	{
-		// ---------------- decision + commit: serial, order dependent ----------------
+		T4AddPlan &plan = sm->plan ;
+		plan.kind = 0 ;
+		plan.seqIdx = -1 ;
+		plan.readInConsensusOffset = 0 ;
+		plan.ret = -1 ;
+		plan.bail = false ;
+		plan.added = false ;
 		T4Ovl *extendedOverlaps = cx.P<T4Ovl>( st->ovlTmpOff ) ;
-		T4Ovl *failedExtendedOverlaps = cx.P<T4Ovl>( st->failOff ) ;
-		int *oldMinExtAnchor = cx.P<int>( st->anchorOff ) ;
-		const int radius = st->radius ;
-		int i, j, k = 0 ;
-		int ret = -1 ;
-		int failedExtendedOverlapsCnt = 0 ;
-		T4Ovl goodExtendedOverlap ;
-		goodExtendedOverlap.seqIdx = -1 ;
-		int readInConsensusOffset = 0 ;
-		int seqIdx = -1 ;
-		int tag = 0 ;
-		bool sortExtendedOverlaps = true ;
-		bool added = false ;
-		bool bail = false ;
-		int kind = 0 ;
-
-		for ( i = 0 ; i < overlapCnt ; ++i )
-		{
-			T4Contig *seq = t4_seq( cx, overlaps[i].seqIdx ) ;
-			oldMinExtAnchor[2 * i] = seq->minLeftExtAnchor ;
-			oldMinExtAnchor[2 * i + 1] = seq->minRightExtAnchor ;
-			for ( j = 0 ; j < k ; ++j )
-			{
-				int leftRadius = radius, rightRadius = radius ;
-				if ( extendedOverlaps[j].seqStart == 0 )
-					leftRadius = 0 ;
-				if ( extendedOverlaps[j].seqEnd == t4_seq( cx, extendedOverlaps[j].seqIdx )->len - 1 )
-					rightRadius = 0 ;
-				if ( overlaps[i].readStart >= extendedOverlaps[j].readStart - leftRadius
-					&& overlaps[i].readEnd <= extendedOverlaps[j].readEnd + rightRadius
-					&& ( overlaps[i].seqStart >= radius || overlaps[i].seqEnd <= seq->len - radius - 1 ) )
-					break ;
-				leftRadius = radius ;
-				rightRadius = radius ;
-				if ( overlaps[i].seqStart == 0 )
-					leftRadius = 0 ;
-				if ( overlaps[i].seqEnd == seq->len - 1 )
-					rightRadius = 0 ;
-				if ( extendedOverlaps[j].readStart >= overlaps[i].readStart - leftRadius
-					&& extendedOverlaps[j].readEnd <= overlaps[i].readEnd + rightRadius )
-					break ;
-			}
-			if ( j < k )
-				continue ;
-			if ( pre[i].hcCnt != 2 )
-				s_make_exact( cx, r, len, factor, overlaps, pre, i ) ;
-			extendedOverlaps[k] = pre[i] ;
-			if ( pre[i].infoFromHits == 1 )
-			{
-				T4Ovl &eo = extendedOverlaps[k] ;
-				if ( eo.similarity < similarityThreshold )
-				{
-					if ( ( minKmerCount <= 1 || eo.similarity + 0.01 >= similarityThreshold ) && eo.readStart == 0
-						&& eo.readEnd == len - 1 )
-						goodExtendedOverlap = eo ;
-					continue ;
-				}
-				for ( j = 0 ; j < k ; ++j )
-				{
-					int leftRadius = radius, rightRadius = radius ;
-					if ( extendedOverlaps[j].seqStart == 0 )
-						leftRadius = 0 ;
-					if ( extendedOverlaps[j].seqEnd == t4_seq( cx, extendedOverlaps[j].seqIdx )->len - 1 )
-						rightRadius = 0 ;
-					if ( eo.readStart >= extendedOverlaps[j].readStart - leftRadius
-						&& eo.readEnd <= extendedOverlaps[j].readEnd + rightRadius
-						&& ( overlaps[i].seqStart > 0 || overlaps[i].seqEnd < seq->len - 1 ) )
-						break ;
-					if ( extendedOverlaps[j].readStart >= eo.readStart - radius && extendedOverlaps[j].readEnd <= eo.readEnd + radius )
-						break ;
-				}
-				if ( j < k )
-					continue ;
-				T4Contig *eseq = t4_seq( cx, eo.seqIdx ) ;
-				int span = eo.readEnd - eo.readStart + 1 ;
-				for ( j = 0 ; j < i ; ++j )
-				{
-					if ( eo.seqStart == 0 && eo.seqEnd == eseq->len - 1 )
-						continue ;
-					if ( eo.readStart >= overlaps[j].readStart && eo.readEnd <= overlaps[j].readEnd
-						&& ( overlaps[j].readEnd - overlaps[j].readStart >= eo.readEnd - eo.readStart + 10
-							|| overlaps[j].similarity + 0.02 >= eo.similarity ) )
-					{
-						if ( eo.readStart > 0 && eseq->minLeftExtAnchor < span )
-							eseq->minLeftExtAnchor = span ;
-						if ( eo.readEnd < len - 1 && eseq->minRightExtAnchor < span )
-							eseq->minRightExtAnchor = span ;
-						break ;
-					}
-				}
-				if ( j < i )
-					continue ;
-				for ( j = 0 ; j < failedExtendedOverlapsCnt ; ++j )
-				{
-					if ( eo.seqStart == 0 && eo.seqEnd == eseq->len - 1 )
-						continue ;
-					if ( eo.readStart >= failedExtendedOverlaps[j].readStart && eo.readEnd <= failedExtendedOverlaps[j].readEnd )
-					{
-						if ( eo.readStart > 0 && eseq->minLeftExtAnchor < span )
-							eseq->minLeftExtAnchor = span ;
-						if ( eo.readEnd < len - 1 && eseq->minRightExtAnchor < span )
-							eseq->minRightExtAnchor = span ;
-						break ;
-					}
-				}
-				if ( j < failedExtendedOverlapsCnt )
-					continue ;
-				if ( eo.readStart > 0 && eseq->minLeftExtAnchor >= span )
-					continue ;
-				if ( eo.readEnd < len - 1 && eseq->minRightExtAnchor >= span )
-					continue ;
-				tag = i ;
-				++k ;
-			}
-			else
-			{
-				failedExtendedOverlaps[failedExtendedOverlapsCnt] = extendedOverlaps[k] ;
-				++failedExtendedOverlapsCnt ;
-			}
-		}
-
-		if ( k == 1 && extendedOverlaps[0].readStart <= radius && extendedOverlaps[0].readEnd >= len - radius )
-		{
-			// could the read bridge to a second contig? (SeqSet.hpp:3732-3793)
-			for ( i = 0 ; i < overlapCnt ; ++i )
-			{
-				if ( tag == i )
-					continue ;
-				if ( pre[i].hcCnt == 1 )
-					continue ; // ExtendOverlap provably returns 0; only the return value is consulted here
-				if ( pre[i].hcCnt != 2 )
-					s_make_exact( cx, r, len, factor, overlaps, pre, i ) ;
-				extendedOverlaps[k] = pre[i] ;
-				if ( pre[i].infoFromHits == 1 )
-				{
-					j = i ;
-					++k ;
-				}
-			}
-			if ( k > 2 )
-				k = 1 ;
-			else if ( k == 2 )
-			{
-				int span = extendedOverlaps[1].readEnd - extendedOverlaps[1].readStart + 1 ;
-				if ( extendedOverlaps[1].readStart > 0 && oldMinExtAnchor[2 * j] >= span )
-					k = 1 ;
-				if ( extendedOverlaps[1].readEnd < len - 1 && oldMinExtAnchor[2 * j + 1] >= span )
-					k = 1 ;
-				if ( k == 2 )
-				{
-					if ( extendedOverlaps[0].seqEnd == t4_seq( cx, extendedOverlaps[0].seqIdx )->len - 1
-						&& extendedOverlaps[1].seqStart == 0 )
-						sortExtendedOverlaps = false ;
-					else if ( extendedOverlaps[0].seqStart == 0
-						&& extendedOverlaps[1].seqEnd == t4_seq( cx, extendedOverlaps[1].seqIdx )->len - 1 )
-					{
-						sortExtendedOverlaps = false ;
-						T4Ovl tmp = extendedOverlaps[0] ;
-						extendedOverlaps[0] = extendedOverlaps[1] ;
-						extendedOverlaps[1] = tmp ;
-					}
-					else
-						k = 1 ;
-				}
-			}
-		}
-
-		if ( similarityThreshold > st->novelSeqSimilarity )
-		{
-			int cnt = 0 ;
-			for ( i = 0 ; i < k ; ++i )
-				if ( extendedOverlaps[i].similarity >= similarityThreshold )
-				{
-					extendedOverlaps[cnt] = extendedOverlaps[i] ;
-					++cnt ;
-				}
-			k = cnt ;
-		}
-		if ( k == 0 && goodExtendedOverlap.seqIdx != -1 )
-		{
-			extendedOverlaps[0] = goodExtendedOverlap ;
-			k = 1 ;
-		}
+		bool sortExtendedOverlaps ;
+		const int k = s_decide_overlaps( cx, overlaps, overlapCnt, r, len, factor, pre, minKmerCount, similarityThreshold,
+			extendedOverlaps, sortExtendedOverlaps ) ;
 		if ( k > 1 )
-		{
-			for ( i = 0 ; i < k ; ++i )
-				if ( extendedOverlaps[i].similarity >= 0.95 )
-					break ;
-			if ( i >= k )
-			{
-				int maxtag = 0 ;
-				for ( i = 1 ; i < k ; ++i )
-					if ( t4_ovl_less( extendedOverlaps[i], extendedOverlaps[maxtag] ) )
-						maxtag = i ;
-				extendedOverlaps[0] = extendedOverlaps[maxtag] ;
-				k = 1 ;
-			}
-		}
-		if ( k > 1 )
-		{
-			for ( i = 0 ; i < k - 1 ; ++i )
-				for ( j = i + 1 ; j < k ; ++j )
-					if ( extendedOverlaps[i].seqIdx == extendedOverlaps[j].seqIdx )
-					{
-						k = 0 ;
-						break ;
-					}
-		}
-
-		if ( k > 1 )
-		{
-			// ------------- merge contigs (SeqSet.hpp:3878-4130); rare (0.7 % of AddReads), serial -------------
-			int eOverlapCnt = k ;
-			added = true ;
-			kind = 2 ;
-			if ( sortExtendedOverlaps )
-			{
-				// std::sort by readStart only; equal keys would make the order implementation defined, so keep the
-				// sort stable and flag ties (they need differing contigs with equal extended read starts)
-				for ( i = 1 ; i < eOverlapCnt ; ++i )
-				{
-					T4Ovl x = extendedOverlaps[i] ;
-					for ( j = i - 1 ; j >= 0 && extendedOverlaps[j].readStart > x.readStart ; --j )
-						extendedOverlaps[j + 1] = extendedOverlaps[j] ;
-					extendedOverlaps[j + 1] = x ;
-				}
-			}
-			for ( i = 0 ; i < k && !bail ; ++i )
-				for ( j = i + 1 ; j < k ; ++j )
-				{
-					T4Contig *ca = t4_seq( cx, extendedOverlaps[i].seqIdx ) ;
-					T4Contig *cb = t4_seq( cx, extendedOverlaps[j].seqIdx ) ;
-					if ( !t4_name_compatible( cx.P<char>( ca->nameOff ), ca->nameLen, cx.P<char>( cb->nameOff ), cb->nameLen ) )
-					{
-						bail = true ;
-						break ;
-					}
-				}
-			if ( bail )
-				ret = -1 ;
-			else
-			{
-				int sum = 0 ;
-				for ( i = 0 ; i < eOverlapCnt ; ++i )
-					sum += t4_seq( cx, extendedOverlaps[i].seqIdx )->len ;
-				// positions of the contigs in the merged contig; extOff (pre[]) is free from here on
-				int *seqOffset = (int *)pre ;
-				if ( extendedOverlaps[0].readStart > 0 )
-				{
-					for ( i = 0 ; i < eOverlapCnt ; ++i )
-						seqOffset[i] = extendedOverlaps[i].readStart ;
-				}
-				else
-				{
-					seqOffset[0] = 0 ;
-					for ( i = 1 ; i < eOverlapCnt ; ++i )
-						seqOffset[i] = seqOffset[i - 1] + t4_seq( cx, extendedOverlaps[i - 1].seqIdx )->len - 1
-							+ ( extendedOverlaps[i].readStart - extendedOverlaps[i - 1].readEnd ) ;
-				}
-				u64 ncOff = s_alloc( cx, (u64)( sum + len + 1 ) + 16 ) ;
-				if ( ncOff )
-				{
-					char *newConsensus = cx.P<char>( ncOff ) ;
-					if ( extendedOverlaps[0].readStart > 0 )
-						memcpy( newConsensus, r, len ) ;
-					else
-						memcpy( newConsensus + extendedOverlaps[0].seqStart, r, len ) ;
-					for ( i = eOverlapCnt - 1 ; i >= 0 ; --i )
-					{
-						T4Contig *c = t4_seq( cx, extendedOverlaps[i].seqIdx ) ;
-						memcpy( newConsensus + seqOffset[i], t4_cons( cx, c ), c->len ) ;
-					}
-					int newConsensusLen = 0 ;
-					int lastEndExtendedOverlapIdx = eOverlapCnt - 1 ;
-					k = 0 ;
-					for ( i = 0 ; i < eOverlapCnt ; ++i )
-					{
-						int e = seqOffset[i] + t4_seq( cx, extendedOverlaps[i].seqIdx )->len ;
-						if ( e > k )
-						{
-							k = e ;
-							lastEndExtendedOverlapIdx = i ;
-						}
-					}
-					if ( extendedOverlaps[lastEndExtendedOverlapIdx].readEnd < len )
-						newConsensusLen = k + ( len - extendedOverlaps[lastEndExtendedOverlapIdx].readEnd - 1 ) ;
-					else
-						newConsensusLen = k ;
-
-					int newSeqIdx = extendedOverlaps[0].seqIdx ;
-					k = 0 ;
-					for ( i = 1 ; i < eOverlapCnt ; ++i )
-						if ( extendedOverlaps[i].seqIdx < newSeqIdx )
-						{
-							newSeqIdx = extendedOverlaps[i].seqIdx ;
-							k = i ;
-						}
-					// index removal uses the OLD consensus of every participant
-					for ( i = 0 ; i < eOverlapCnt ; ++i )
-					{
-						T4Contig *c = t4_seq( cx, extendedOverlaps[i].seqIdx ) ;
-						s_remove_index( cx, t4_cons( cx, c ), c->len, extendedOverlaps[i].seqIdx, barcode, 0 ) ;
-					}
-					// new posWeight: old columns of newSeqIdx shifted by seqOffset[k], zero elsewhere, plus the others
-					T4Contig *ns = t4_seq( cx, newSeqIdx ) ;
-					int oldLen = ns->len ;
-					int cap = 2 * newConsensusLen + 128 ;
-					u64 co = s_alloc( cx, cap ) ;
-					u64 po = s_alloc( cx, T4_PW_BYTES( cap ) ) ;
-					if ( co && po )
-					{
-						int lead = ( cap - newConsensusLen ) / 2 ;
-						int *npw = cx.P<int>( po ) + 4 * lead ;
-						unsigned char *neq = cx.P<unsigned char>( po + 16ull * cap ) + lead ;
-						int *opw = t4_pw( cx, ns ) ;
-						for ( i = 0 ; i < 4 * newConsensusLen ; ++i )
-							npw[i] = 0 ;
-						for ( i = 0 ; i < 4 * oldLen ; ++i )
-							npw[4 * seqOffset[k] + i] = opw[i] ;
-						for ( i = 0 ; i < eOverlapCnt ; ++i )
-						{
-							int sIdx = extendedOverlaps[i].seqIdx ;
-							if ( sIdx == newSeqIdx )
-								continue ;
-							T4Contig *c = t4_seq( cx, sIdx ) ;
-							ns->numRead += c->numRead ;
-							int *cpw = t4_pw( cx, c ) ;
-							for ( j = 0 ; j < 4 * c->len ; ++j )
-								npw[4 * seqOffset[i] + j] += cpw[j] ;
-						}
-						for ( i = 0 ; i < newConsensusLen ; ++i )
-							neq[i] = (unsigned char)t4_eq_nibble( npw + 4 * i ) ;
-						// name (SeqSet.hpp:4066-4096)
-						int nameIdx ;
-						for ( nameIdx = 0 ; nameIdx < eOverlapCnt ; ++nameIdx )
-						{
-							T4Contig *c = t4_seq( cx, extendedOverlaps[nameIdx].seqIdx ) ;
-							if ( !t4_name_eq( cx.P<char>( c->nameOff ), c->nameLen, "Novel", 5 ) )
-								break ;
-						}
-						if ( nameIdx >= eOverlapCnt )
-							nameIdx = 0 ;
-						int nameSum = 0 ;
-						for ( i = 0 ; i < eOverlapCnt ; ++i )
-							nameSum += t4_seq( cx, extendedOverlaps[i].seqIdx )->nameLen ;
-						u64 nbOff = s_alloc( cx, nameSum + eOverlapCnt + 1 ) ;
-						if ( nbOff )
-						{
-							char *nameBuffer = cx.P<char>( nbOff ) ;
-							T4Contig *c0 = t4_seq( cx, extendedOverlaps[nameIdx].seqIdx ) ;
-							memcpy( nameBuffer, cx.P<char>( c0->nameOff ), c0->nameLen ) ;
-							int nl = c0->nameLen ;
-							for ( i = 0 ; i < eOverlapCnt ; ++i )
-							{
-								if ( i == nameIdx )
-									continue ;
-								if ( i > 0 )
-								{
-									T4Contig *ci = t4_seq( cx, extendedOverlaps[i].seqIdx ) ;
-									T4Contig *cp = t4_seq( cx, extendedOverlaps[i - 1].seqIdx ) ;
-									if ( !t4_name_eq( cx.P<char>( ci->nameOff ), ci->nameLen, cx.P<char>( cp->nameOff ), cp->nameLen ) )
-									{
-										nameBuffer[nl] = '+' ;
-										memcpy( nameBuffer + nl + 1, cx.P<char>( ci->nameOff ), ci->nameLen ) ;
-										nl += 1 + ci->nameLen ;
-									}
-								}
-							}
-							nameBuffer[nl] = '\0' ;
-							int minLeft = t4_seq( cx, extendedOverlaps[0].seqIdx )->minLeftExtAnchor ;
-							int minRight = t4_seq( cx, extendedOverlaps[lastEndExtendedOverlapIdx].seqIdx )->minRightExtAnchor ;
-							// release the merged-away contigs (SeqSet::ReleaseSeq: the slot stays, NULL consensus)
-							for ( i = 0 ; i < eOverlapCnt ; ++i )
-							{
-								int sIdx = extendedOverlaps[i].seqIdx ;
-								if ( sIdx == newSeqIdx )
-									continue ;
-								T4Contig *c = t4_seq( cx, sIdx ) ;
-								c->consOff = 0 ;
-								c->pwOff = 0 ;
-								c->nameOff = 0 ;
-								c->len = 0 ;
-							}
-							ns->nameOff = nbOff ;
-							ns->nameLen = nl ;
-							ns->consOff = co ;
-							ns->pwOff = po ;
-							ns->cap = cap ;
-							ns->lead = lead ;
-							ns->len = newConsensusLen ;
-							memcpy( t4_cons( cx, ns ), newConsensus, newConsensusLen ) ;
-							s_update_consensus( cx, newSeqIdx, false ) ;
-							s_build_index( cx, t4_cons( cx, ns ), newConsensusLen, newSeqIdx, barcode, 0 ) ;
-							ns->minLeftExtAnchor = minLeft ;
-							ns->minRightExtAnchor = minRight ;
-							readInConsensusOffset = 0 ;
-							if ( extendedOverlaps[0].seqStart > 0 )
-								readInConsensusOffset = extendedOverlaps[0].seqStart ;
-							seqIdx = newSeqIdx ;
-						}
-					}
-				}
-			}
-		}
+			s_merge_commit( cx, extendedOverlaps, k, sortExtendedOverlaps, r, len, barcode, (int *)pre, plan ) ;
 		else if ( k == 1 )
 		{
-			added = true ;
-			kind = 1 ;
-			sm->e0 = extendedOverlaps[0] ;
+			plan.added = true ;
+			plan.kind = 1 ;
+			plan.e0 = extendedOverlaps[0] ;
 		}
-		sm->bi[2] = kind ;
-		sm->bi[3] = seqIdx ;
-		sm->bi[4] = readInConsensusOffset ;
-		sm->bi[5] = bail ? 1 : 0 ;
-		sm->bi[6] = ret ;
-		sm->bi[7] = added ? 1 : 0 ;
 	}
 	T4_SYNC() ;
-	int kind = sm->bi[2] ;
-	int seqIdx = sm->bi[3] ;
-	int readInConsensusOffset = sm->bi[4] ;
-	bool bail = sm->bi[5] != 0 ;
-	int ret = sm->bi[6] ;
-	bool added = sm->bi[7] != 0 ;
-	T4_SYNC() ;
-	if ( kind == 1 )
+	T4AddPlan p = sm->plan ;
+	if ( p.kind == 1 )
+		c_extend_commit( cx, p, r, len, barcode, minKmerCount, (char *)pre ) ;
+	if ( p.added && !p.bail && p.seqIdx >= 0 && !st->error )
 	{
-		// ------------- extend / inside a contig (SeqSet.hpp:4131-4316); collective -------------
-		const T4Ovl e0 = sm->e0 ;
-		seqIdx = e0.seqIdx ;
-		T4Contig *seq = t4_seq( cx, seqIdx ) ;
-		if ( cx.tid == 0 )
-			++seq->numRead ;
-		if ( e0.readStart > 0 || e0.readEnd < len - 1 )
-		{
-			const int shift = e0.readStart ;
-			const int rightAdd = ( e0.readEnd < len - 1 ) ? ( len - 1 - e0.readEnd ) : 0 ;
-			const int oldLen = seq->len ;
-			const int kl = st->kmerLength ;
-			// index first, in the reference's order: new left k-mers, shift the old postings, (later) new right k-mers
-			if ( shift > 0 )
-			{
-				char *oldCons = t4_cons( cx, seq ) ;
-				char *tmpc = (char *)pre ; // newConsensus[0 .. shift + kl - 1): read prefix + the first kl-1 old bases
-				int n = shift + kl - 1 ;
-				T4_PAR_FOR( i, n )
-				{
-					char c ;
-					if ( i < shift )
-						c = r[i] ;
-					else if ( i - shift < oldLen )
-						c = oldCons[i - shift] ;
-					else
-					{
-						int ri = e0.readEnd + 1 + ( i - shift - oldLen ) ;
-						c = ( ri < len ) ? r[ri] : '\0' ;
-					}
-					tmpc[i] = c ;
-				}
-				T4_SYNC() ;
-				c_index_op( cx, tmpc, n, T4_IDX_BUILD, seqIdx, barcode, 0, 0 ) ;
-				c_index_op( cx, oldCons, oldLen, T4_IDX_UPDATE, seqIdx, barcode, shift, seqIdx ) ;
-			}
-			T4_SYNC() ; // every thread has read the old length / pointers
-			if ( cx.tid == 0 )
-				sm->bi[0] = s_contig_grow( cx, seq, shift, rightAdd ) ? 1 : 0 ;
-			T4_SYNC() ;
-			bool grown = sm->bi[0] != 0 ;
-			T4_SYNC() ;
-			if ( !grown )
-			{
-				ret = T4_E_NOMEM ;
-				bail = true ;
-			}
-			else
-			{
-				char *newConsensus = t4_cons( cx, seq ) ;
-				int *pw = t4_pw( cx, seq ) ;
-				unsigned char *eq = t4_eq( cx, seq ) ;
-				const int newConsensusLen = seq->len ;
-				T4_PAR_FOR( i, shift )
-					newConsensus[i] = r[i] ;
-				T4_PAR_FOR( x, rightAdd )
-					newConsensus[shift + oldLen + x] = r[e0.readEnd + 1 + x] ;
-				T4_PAR_FOR( i, shift )
-					t4_col_put( pw, eq, i, 0, 0, 0, 0 ) ;
-				T4_PAR_FOR( i, rightAdd )
-					t4_col_put( pw, eq, shift + oldLen + i, 0, 0, 0, 0 ) ;
-				T4_SYNC() ;
-				if ( e0.readEnd < len - 1 )
-				{
-					int start = e0.readStart + e0.seqEnd - kl + 2 ;
-					if ( start < 0 )
-					{
-						if ( cx.tid == 0 )
-							t4_raise( cx, T4_E_INTERNAL, 11 ) ;
-						start = 0 ;
-					}
-					c_index_op( cx, newConsensus + start, newConsensusLen - start, T4_IDX_BUILD, seqIdx, barcode, start, 0 ) ;
-				}
-				// end-weight decay and scheduled consensus substitutions (SeqSet.hpp:4192-4247): four columns, serial
-				if ( cx.tid == 0 )
-				{
-					int nrep = 0 ;
-					if ( shift > 0 && ( barcode == -1 || minKmerCount > 1 ) )
-					{
-						for ( int i = 0 ; i < 2 ; ++i )
-						{
-							if ( i + shift >= len || r[i + shift] == 'N' )
-								continue ;
-							char nc = newConsensus[i + shift] ;
-							if ( r[i + shift] != nc && nc != 'N' && pw[4 * ( i + shift ) + t4_nuc( nc )] == 1 )
-							{
-								sm->bi[2 + nrep] = i + shift ;
-								sm->bi[6 + nrep] = r[i + shift] ;
-								++nrep ;
-							}
-							for ( int j = 0 ; j < 4 ; ++j )
-								if ( r[i + shift] != t4_numToNuc( j ) && pw[4 * ( i + shift ) + j] > 1 )
-									t4_col_add( pw, eq, i + shift, j, -1 ) ;
-						}
-					}
-					if ( e0.readEnd < len - 1 && ( barcode == -1 || minKmerCount > 1 ) )
-					{
-						for ( int i = oldLen - 2 ; i < oldLen ; ++i )
-						{
-							int pos = i - e0.seqStart ;
-							int seqPos = i + shift ;
-							if ( pos < 0 || r[pos] == 'N' )
-								continue ;
-							if ( i < 0 )
-							{
-								t4_raise( cx, T4_E_INTERNAL, 12 ) ;
-								continue ;
-							}
-							char nc = newConsensus[seqPos] ;
-							if ( r[pos] != nc && nc != 'N' && pw[4 * seqPos + t4_nuc( nc )] == 1 )
-							{
-								sm->bi[2 + nrep] = seqPos ;
-								sm->bi[6 + nrep] = r[pos] ;
-								++nrep ;
-							}
-							for ( int j = 0 ; j < 4 ; ++j )
-								if ( r[pos] != t4_numToNuc( j ) && pw[4 * seqPos + j] > 1 )
-									t4_col_add( pw, eq, seqPos, j, -1 ) ;
-						}
-					}
-					if ( shift > 0 )
-						seq->minLeftExtAnchor = 0 ;
-					if ( e0.readEnd < len - 1 )
-						seq->minRightExtAnchor = 0 ;
-					sm->bi[1] = nrep ;
-				}
-				T4_SYNC() ;
-				// (the +GENE name adjustment needs isRef overlaps: never in the stage-1 novel set, SeqSet.hpp:4258-4296)
-				readInConsensusOffset = 0 ;
-				if ( e0.seqStart > 0 )
-					readInConsensusOffset = e0.seqStart ;
-				int nrep = sm->bi[1] ;
-				int repPos[4], repChar[4] ;
-				for ( int i = 0 ; i < nrep ; ++i )
-				{
-					repPos[i] = sm->bi[2 + i] ;
-					repChar[i] = sm->bi[6 + i] ;
-				}
-				T4_SYNC() ;
-				for ( int i = 0 ; i < nrep ; ++i )
-					c_substitute_consensus_pos( cx, seqIdx, repPos[i], (char)repChar[i] ) ;
-			}
-		}
-		else
-			readInConsensusOffset = e0.seqStart ;
-	}
-
-	// ------------- posWeight update (SeqSet.hpp:4318-4363); collective -------------
-	if ( added && !bail && seqIdx >= 0 && !st->error )
-	{
-		T4Contig *seq = t4_seq( cx, seqIdx ) ;
-		char *cons = t4_cons( cx, seq ) ;
-		int *pw = t4_pw( cx, seq ) ;
-		unsigned char *eq = t4_eq( cx, seq ) ;
-		if ( cx.tid == 0 )
-			sm->bi[0] = 0 ;
-		T4_SYNC() ;
-		T4_PAR_FOR( i, len )
-		{
-			if ( r[i] == 'N' )
-				continue ;
-			t4_col_add( pw, eq, i + readInConsensusOffset, t4_nuc( r[i] ), 1 ) ;
-			if ( cons[i + readInConsensusOffset] == 'N' )
-				sm->bi[0] = 1 ;
-		}
-		T4_SYNC() ;
-		if ( cx.tid == 0 )
-		{
-			t4_set_prev( st, seqIdx, 0, len - 1, readInConsensusOffset, overlaps[0].strand ) ;
-			if ( sm->bi[0] )
-			{
-				// consensus N's under the read are filled and their k-mers indexed (SeqSet.hpp:4338-4360); rare
-				int kl = st->kmerLength ;
-				int *nPos = (int *)pre ;
-				int size = 0 ;
-				for ( int i = 0 ; i < len ; ++i )
-					if ( r[i] != 'N' && cons[i + readInConsensusOffset] == 'N' )
-						nPos[size++] = i ;
-				for ( int i = 0 ; i < size ; )
-				{
-					int j ;
-					for ( j = i + 1 ; j < size ; ++j )
-						if ( nPos[j] > nPos[j - 1] + kl - 1 )
-							break ;
-					for ( int l = i ; l < j ; ++l )
-						cons[nPos[l] + readInConsensusOffset] = r[nPos[l]] ;
-					int start = nPos[i] - kl + 1 + readInConsensusOffset ;
-					if ( start < 0 )
-						start = 0 ;
-					int end = nPos[j - 1] + kl - 1 + readInConsensusOffset ;
-					if ( end >= seq->len )
-						end = seq->len - 1 ;
-					s_build_index( cx, cons + start, end - start + 1, seqIdx, barcode, start ) ;
-					i = j ;
-				}
-			}
-		}
-		ret = seqIdx ;
+		c_posweight_update( cx, p.seqIdx, p.readInConsensusOffset, r, len, barcode, overlaps[0].strand, (int *)pre ) ;
+		p.ret = p.seqIdx ;
 	}
 	// addNew is only kept for isRef overlaps (SeqSet.hpp:4377-4391): never in the novel set
-	if ( ret == -1 && !bail )
+	if ( p.ret == -1 && !p.bail )
 	{
 		if ( cx.tid == 0 )
 			t4_set_prev( st, -2, -1, -1, -1, 0 ) ;
-		ret = -2 ;
+		p.ret = -2 ;
 	}
-	if ( ret >= 0 && strand == 0 )
+	if ( p.ret >= 0 && strand == 0 )
 		strand = overlaps[0].strand ;
 	T4_SYNC() ;
 	T4_PHASE( cx, 0 ) ;
 	if ( st->error )
 		return st->error ;
-	return ret ;
+	return p.ret ;
 }
 
 
