@@ -143,7 +143,7 @@ int t4_dp_pos_weight_batch(int n, const int32_t *t_weights, const int64_t *t_off
 
 /* The same alignment through the two routines the stream kernel actually runs for its equal-length problems
  * (overhangs of ExtendOverlap, SeqSet.hpp:1165; same-diagonal gaps of GetOverlapsFromRead, SeqSet.hpp:1832-2006):
- * variant 0 = per-thread register banded DP, variant 1 = half-warp anti-diagonal DP (no <=2-mismatch fast path:
+ * variant 0 = per-thread register banded DP, variant 1 = half-warp row-per-step DP (no <=2-mismatch fast path:
  * its caller settles those from popcounts), variant 2 = ExtendOverlap's overhang pass: problems 2k and 2k+1 run on the
  * two halves of one warp as a left overhang (statistics taken from its end) and a right one, and instead of the edit
  * string align_out receives at align_off[i] (a multiple of 4, 16 bytes) four int32: the matches, mismatches and indels

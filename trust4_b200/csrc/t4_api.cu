@@ -165,7 +165,7 @@ __global__ void t4_pack_kernel( char *A, const u64 *streamOff, const u64 *outOff
 
 // Test entry for the two DP routines the stream kernel really runs (equal lengths: overhangs and same-diagonal gaps):
 // variant 0 = t4_dp_equal (register-resident banded DP, one thread per problem, ExtendOverlap),
-// variant 1 = w_stage_side + w_dp_equal_half (half-warp anti-diagonal DP over staged IsBaseEqual nibbles, gap scoring;
+// variant 1 = w_stage_side + w_dp_equal_half (half-warp row-per-step DP over staged IsBaseEqual nibbles, gap scoring;
 //             it has no fast path: the caller only runs it when the diagonal has > 2 mismatches),
 // variant 2 = w_side_pair (ExtendOverlap's overhang pass: problems 2k and 2k+1 on the two halves of warp k, as a left
 //             side, scanned from its end, and a right side); writes each problem's T4SideStats, not its edit string.

@@ -2733,9 +2733,24 @@ T4_D inline int t4_extend_overlap( T4Ctx &cx, const char *r, int len, T4Contig *
 // ---------------------------------------------------------------------------
 #define T4_FULL 0xffffffffu
 
-// Banded DP for equal lengths in a HALF warp: the 16 lanes own the 13 window slots, anti-diagonal schedule
-// T = 2 i + slot (cell (i, slot) needs (i-1, slot) at T-2 and (i, slot-1), (i-1, slot+1) at T-1, which are the
-// neighbours' most recent values, exchanged by shuffles).  All 32 lanes call; a half with n == 0 idles.
+// Banded DP for equal lengths in a HALF warp, one matrix row per step: lane s < 13 of the half owns window slot s, the
+// cell (i, j = i - 6 + s) of row i.  H(i, j) = max( dg, up, lf ) with dg = H(i-1, j-1) + diff (the lane's own value of
+// the previous row), up = H(i-1, j) + g (slot s + 1 of the previous row, one shuffle) and lf = H(i, j-1) + g, g =
+// SCORE_INDEL, the only dependence inside a row.  Column 0 holds (i + 1) g, other cells outside the band negInf; lanes
+// 13-15, and every lane of a half whose rows are done, keep their values.  All 32 lanes call; a half with n == 0 idles.
+//
+// The left moves are settled after the rest of the row.  Let D = max( dg, up ) in an in-band cell and D = H elsewhere
+// (the fixed values above).  Then H(j) = max( D(j), H(j-1) + g ) in the band and H = D outside it.
+//  - If no in-band cell has D(j-1) + g > D(j), then H = D in the whole row.  This follows by induction from slot 0, which
+//    is never in the band.  That is the common row, and it costs one vote.
+//  - Otherwise H(j) = max over k <= j of D(k) + (j - k) g, where k runs down to the slot left of the row's first in-band
+//    cell: that slot is column 0 or out of the band, so its H is its fixed value and the chain stops there.  The
+//    inclusive max-plus scan over the half's slots computes this maximum, plus terms for slots further left.  Those
+//    slots hold negInf, so each extra term is at most negInf + 2 g = -4 (n + 1)^2 - 8.  Every in-band H is at least the
+//    score of its diagonal path from row 0 or column 0, (d + 1) g - 2 n >= -6 n for its offset d = |i - j| <= n - 1.
+//    So the extra terms never win, and the scan gives exactly H.
+// The edit code needs no lf: when H equals neither dg nor up, it equals lf.  So every value, edit code and traceback word
+// is the one of the cell-by-cell recurrence (t4_dp_equal).
 // nib: the IsBaseEqual nibbles of the n target columns, 8 per word (staged in shared memory by w_stage_side), so the
 // loop touches no global memory.  actBase / actStride: traceback words of slot s at actBase + s * actStride.
 // Returns the score in every lane of the half; the half's lane 0 writes the edit string to `align`; *alignLen = its length.
@@ -2746,49 +2761,57 @@ T4_D inline int w_dp_equal_half( T4Ctx &cx, const u32 *nib, const char *p, int n
 	const int nmax = max( n, __shfl_xor_sync( T4_FULL, n, 16 ) ) ;
 	const int negInf = ( n + 1 ) * ( n + 1 ) * SCORE_INDEL ;
 	const int j0 = hl - 6 ;
-	int latest = ( j0 == 0 ) ? 0 : ( j0 > 0 ? SCORE_INDEL + j0 * SCORE_INDEL : negInf ) ;
+	int h = ( j0 == 0 ) ? 0 : ( j0 > 0 ? SCORE_INDEL + j0 * SCORE_INDEL : negInf ) ;
 	u32 *myAct = actBase + hl * actStride ;
 	u32 aw = 0 ;
-	for ( int T = 2 ; T <= 2 * nmax + 12 ; ++T )
+	// IsBaseEqual of the lane's column in row r + 1 (column r - 6 + hl, read base p[r]), for r < n; it is loaded a row
+	// ahead so that it stays off the H chain
+	auto eqOfRow = [&]( int r ) -> bool {
+		const int c = r - 6 + hl ;
+		const char pc = p[r] ;
+		const u32 nb = ( (unsigned)c < (unsigned)n ) ? nib[c >> 3] >> ( 4 * ( c & 7 ) ) : 0u ;
+		return ( pc == 'N' ) || ( ( nb >> t4_nuc( pc ) ) & 1u ) ;
+	} ;
+	bool eqNext = n > 0 && eqOfRow( 0 ) ;
+	for ( int i = 1 ; i <= nmax ; ++i )
 	{
-		int vl = __shfl_up_sync( T4_FULL, latest, 1, 16 ) ;
-		int vu = __shfl_down_sync( T4_FULL, latest, 1, 16 ) ;
-		int i = ( T - hl ) >> 1 ;
-		if ( hl < 13 && ( ( T - hl ) & 1 ) == 0 && i >= 1 && i <= n )
+		const bool eq = eqNext ;
+		if ( i < n )
+			eqNext = eqOfRow( i ) ;
+		const int j = i - 6 + hl ;
+		const bool live = hl < 13 && i <= n ;
+		const bool inBand = live && (unsigned)( hl - 1 ) < 11u && (unsigned)( j - 1 ) < (unsigned)n ;
+		const int dg = h + ( eq ? SCORE_MATCH : SCORE_MISMATCH ) ;
+		const int up = __shfl_down_sync( T4_FULL, h, 1, 16 ) + SCORE_INDEL ;
+		if ( inBand )
+			h = max( dg, up ) ;
+		else if ( live )
+			h = ( j == 0 ) ? SCORE_INDEL + i * SCORE_INDEL : negInf ;
+		const int lf = __shfl_up_sync( T4_FULL, h, 1, 16 ) + SCORE_INDEL ;
+		if ( __any_sync( T4_FULL, inBand && lf > h ) )
 		{
-			int j = i - 6 + hl ;
-			int start = i - 5 < 1 ? 1 : i - 5 ;
-			int end = i + 5 > n ? n : i + 5 ;
-			int val ;
+			// a lane below its shift gets its own value back, and s + k g < s
+			int s = h ;
+#pragma unroll
+			for ( int k = 1 ; k < 16 ; k <<= 1 )
+				s = max( s, __shfl_up_sync( T4_FULL, s, k, 16 ) + k * SCORE_INDEL ) ;
+			if ( inBand )
+				h = s ;
+		}
+		if ( live )
+		{
 			u32 a = 0 ;
-			if ( j == 0 )
-				val = SCORE_INDEL + i * SCORE_INDEL ;
-			else if ( j < start || j > end )
-				val = negInf ;
-			else
-			{
-				char pc = p[i - 1] ;
-				u32 nb = ( nib[( j - 1 ) >> 3] >> ( 4 * ( ( j - 1 ) & 7 ) ) ) & 15u ;
-				bool eq = ( pc == 'N' ) || ( ( nb >> t4_nuc( pc ) ) & 1u ) ;
-				int diff = eq ? SCORE_MATCH : SCORE_MISMATCH ;
-				int dg = latest + diff, lf = vl + SCORE_INDEL, up = vu + SCORE_INDEL ;
-				val = dg ;
-				if ( lf > val ) val = lf ;
-				if ( up > val ) val = up ;
-				if ( lf == val ) a = EDIT_DELETE ;
-				if ( up == val ) a = EDIT_INSERT ;
-				if ( dg == val ) a = eq ? EDIT_MATCH : EDIT_MISMATCH ;
-			}
+			if ( inBand )
+				a = ( dg == h ) ? ( eq ? (u32)EDIT_MATCH : (u32)EDIT_MISMATCH ) : ( ( up == h ) ? (u32)EDIT_INSERT : (u32)EDIT_DELETE ) ;
 			aw |= a << ( 2 * ( i & 15 ) ) ;
 			if ( ( i & 15 ) == 15 || i == n )
 			{
 				myAct[i >> 4] = aw ;
 				aw = 0 ;
 			}
-			latest = val ;
 		}
 	}
-	int ret = __shfl_sync( T4_FULL, latest, 6, 16 ) ;
+	int ret = __shfl_sync( T4_FULL, h, 6, 16 ) ;
 	__syncwarp() ;
 	int tag = 0 ;
 	if ( hl == 0 && n > 0 )
