@@ -12,8 +12,10 @@
 // STATUS: verified on an H100 against the compiled reference through t4_refset_get_overlaps and t4_refset_annotate
 // (tests/test_gpu_preprocess.py: 528 workers on one read cursor, batch sizes around the worker count, the shipped example
 // on the reference's hg38 gene set, interleaved scan / annotate / get-overlaps calls), and through the test emulation.  It
-// runs in a kernel of its own (t4_annot_kernel).  Probe and key sort are the engine's collectives; everything after is
-// serial per read on thread 0 in plain C (shared with the emulation).
+// runs in a kernel of its own (t4_annot_kernel).  Probe and key sort are the engine's collectives (c_ref_sorted_hits);
+// everything after is serial per read on thread 0 in plain C (shared with the emulation).  The chain walk of a bucket is
+// the stage-0 scan's t4_ref_bucket_chains (t4_refscan.h); overlaps are the engine's T4Ovl with its order, low-complexity
+// and gene-name rules.
 #ifndef T4_ANNOT_H
 #define T4_ANNOT_H
 
@@ -22,26 +24,12 @@
 #define SCORE_GAPOPEN (-4)
 #define SCORE_GAPEXTEND (-1)
 
-struct T4ROvl              // struct _overlap (SeqSet.hpp:76) with its hitCoords as a range of the chain pool
-{
-	int seqIdx ;
-	int readStart, readEnd ;
-	int seqStart, seqEnd ;
-	int strand ;
-	int matchCnt ;
-	int indelCnt ;
-	double similarity ;
-	int hcStart, hcCnt ;
-	int infoFromHits ;
-	int pad ;
-} ;
-
 struct T4AnnotScratch      // serial work space of one read (global memory), carved from one block by t4_annot_carve
 {
 	T4ScanScratch S ;      // bucket / window / LIS arrays (t4_refscan.h)
 	int *hcA, *hcB ;       // chain pool: hitCoords of all overlaps
 	int hcCap, hcUsed ;
-	T4ROvl *ovl, *ovlTmp, *acc ; // acc: the overlaps of all contigs of a read (AnnotateRead)
+	T4Ovl *ovl, *ovlTmp, *acc ; // acc: the overlaps of all contigs of a read (AnnotateRead)
 	int ovlCap ;
 	int *seqUsed ;         // int[nSeqs]
 	int *ca, *cb ;         // contig intervals of the read (64 each)
@@ -56,7 +44,7 @@ T4_HD inline size_t t4_annot_scratch_bytes( int H, int gapLimit, int readLen, in
 {
 	const size_t h = (size_t)( H > 16 ? H : 16 ) ;
 	const size_t g = (size_t)( gapLimit + 2 ) ;
-	return 1024 + 8 * ( 2 * h ) + 4 * ( 6 * h ) + 4 * ( 2 * h ) + 3 * sizeof( T4ROvl ) * h + 8 * h + 3 * 4 * g * g + ( 2 * g + 2 * (size_t)readLen + 64 )
+	return 1024 + 8 * ( 2 * h ) + 4 * ( 6 * h ) + 4 * ( 2 * h ) + 3 * sizeof( T4Ovl ) * h + 8 * h + 3 * 4 * g * g + ( 2 * g + 2 * (size_t)readLen + 64 )
 		+ 4 * (size_t)( nSeqs + 4 ) + 4 * 128 ;
 }
 
@@ -72,9 +60,9 @@ T4_HD inline void t4_annot_carve( T4AnnotScratch &X, char *base, int H, int gapL
 	X.hcB = (int *)p ; p += 4 * h ;
 	X.hcCap = (int)h ; X.hcUsed = 0 ;
 	p = (char *)( ( (uintptr_t)p + 15 ) & ~(uintptr_t)15 ) ;
-	X.ovl = (T4ROvl *)p ; p += sizeof( T4ROvl ) * h ;
-	X.ovlTmp = (T4ROvl *)p ; p += sizeof( T4ROvl ) * h ;
-	X.acc = (T4ROvl *)p ; p += sizeof( T4ROvl ) * h ;
+	X.ovl = (T4Ovl *)p ; p += sizeof( T4Ovl ) * h ;
+	X.ovlTmp = (T4Ovl *)p ; p += sizeof( T4Ovl ) * h ;
+	X.acc = (T4Ovl *)p ; p += sizeof( T4Ovl ) * h ;
 	X.ovlCap = (int)h ;
 	X.seqUsed = (int *)p ; p += 4 * (size_t)( nSeqs + 4 ) ;
 	X.ca = (int *)p ; p += 4 * 64 ;
@@ -100,19 +88,32 @@ struct T4RefView
 	double refSeqSimilarity ;
 	T4_HD const char *cons( int idx ) const { return A + seqs[idx].consOff + seqs[idx].lead ; }
 	T4_HD const char *name( int idx ) const { return A + seqs[idx].nameOff ; }
+	T4_HD int nameLen( int idx ) const { return seqs[idx].nameLen ; }
 	T4_HD int len( int idx ) const { return seqs[idx].len ; }
 } ;
 
-T4_HD inline int t4_rk_a( u64 k ) { return (int)( ( k >> 30 ) & 0x7ff ) ; }        // re-keyed hit (t4_refscan.h): read offset
-T4_HD inline int t4_rk_b( u64 k ) { return (int)( ( k >> 1 ) & T4_KEY_B_MASK ) ; } // gene offset
+// the view of the gene set cx is attached to
+T4_D inline T4RefView t4_ref_view( T4Ctx &cx )
+{
+	const T4Stream *st = cx.st ;
+	T4RefView V ;
+	V.seqs = cx.P<T4Contig>( st->seqsOff ) ;
+	V.A = cx.A ;
+	V.nSeqs = st->nSeqs ;
+	V.k = st->kmerLength ;
+	V.radius = st->radius ;
+	V.hitLenRequired = st->hitLenRequired ;
+	V.nomatchGapLimit = st->nomatchGapLimit ;
+	V.refSeqSimilarity = 0.75 ; // SeqSet.hpp:2566
+	return V ;
+}
 
-// SeqSet::GetOverlapsFromHits for hits on reference sequences (SeqSet.hpp:763-1063): keys sorted by (strand, gene, a, b).
-// filter / conservativeChain have no effect on a pure reference set (the filter statistics count novel sequences only and
-// every posting list is below the `repeats` limit; conservativeChain is false for readType 0).  Appends to X.ovl from
-// `first`; returns the new count.
+// SeqSet::GetOverlapsFromHits for hits on reference sequences (SeqSet.hpp:763-1063): keys sorted by (strand, gene, a, b),
+// each (strand, gene) bucket chained by t4_ref_bucket_chains.  filter / conservativeChain have no effect on a pure reference
+// set (the filter statistics count novel sequences only and every posting list is below the `repeats` limit;
+// conservativeChain is false for readType 0).  Appends to X.ovl from `first`; returns the new count.
 T4_HD inline int t4_ref_overlaps_from_hits( const u64 *keys, int H, const T4RefView &V, int hitLenRequired, T4AnnotScratch &X, int first )
 {
-	const int minHitRequired = 3 ;
 	int n = first ;
 	for ( int i = 0 ; i < H ; )
 	{
@@ -120,83 +121,36 @@ T4_HD inline int t4_ref_overlaps_from_hits( const u64 *keys, int H, const T4RefV
 		int j = i + 1 ;
 		while ( j < H && ( keys[j] >> T4_KEY_IDX_SHIFT ) == g )
 			++j ;
-		const int cnt = j - i ;
-		if ( cnt >= minHitRequired )
-		{
-			u64 *w = X.S.w ;
-			for ( int x = 0 ; x < cnt ; ++x )
+		const bool walked = t4_ref_bucket_chains( keys + i, j - i, V.k, V.radius, hitLenRequired, X.S, [&]( int lisSize, int hitLen ) {
+			if ( n >= X.ovlCap || X.hcUsed + lisSize > X.hcCap )
 			{
-				const int a = t4_rk_a( keys[i + x] ), b = t4_rk_b( keys[i + x] ) ;
-				w[x] = ( (u64)( a - b + T4_KEY_C_BIAS ) << 40 ) | ( (u64)b << 20 ) | (u64)a ;
+				X.overflow = 1 ;
+				return false ;
 			}
-			t4_heapsort64( w, cnt ) ;
-			for ( int s = 0 ; s < cnt ; )
+			T4Ovl &no = X.ovl[n] ;
+			no.seqIdx = t4_key_idx( keys[i] ) ;
+			no.readStart = X.S.oa[0] ;
+			no.readEnd = X.S.oa[lisSize - 1] + V.k - 1 ;
+			no.strand = t4_key_strand( keys[i] ) ;
+			no.seqStart = X.S.ob[0] ;
+			no.seqEnd = X.S.ob[lisSize - 1] + V.k - 1 ;
+			no.matchCnt = 2 * hitLen ;
+			no.indelCnt = 0 ;
+			no.similarity = 0 ;
+			no.hcStart = X.hcUsed ;
+			no.hcCnt = lisSize ;
+			no.infoFromHits = 0 ;
+			for ( int x = 0 ; x < lisSize ; ++x )
 			{
-				int e ;
-				for ( e = s + 1 ; e < cnt ; ++e )
-				{
-					int diff = (int)( w[e] >> 40 ) - (int)( w[e - 1] >> 40 ) ;
-					if ( diff < 0 )
-						diff = -diff ;
-					if ( diff > V.radius )
-						break ;
-				}
-				if ( e - s < minHitRequired || ( e - s ) * V.k < hitLenRequired )
-				{
-					s = e ;
-					continue ;
-				}
-				const int m = e - s ;
-				u64 *cw = w + cnt ;
-				for ( int x = 0 ; x < m ; ++x )
-					cw[x] = w[s + x] & ( ( 1ull << 40 ) - 1ull ) ;
-				if ( V.radius > 0 )
-					t4_heapsort64( cw, m ) ;
-				for ( int x = 0 ; x < m ; ++x )
-				{
-					X.S.ha[x] = (int)( cw[x] & 0xfffff ) ;
-					X.S.hb[x] = (int)( cw[x] >> 20 ) ;
-				}
-				const int lisSize = t4_lis( X.S.ha, X.S.hb, m, X.S.top, X.S.link, X.S.oa, X.S.ob ) ;
-				if ( lisSize * V.k < hitLenRequired )
-				{
-					s = e ;
-					continue ;
-				}
-				const int hitLen = t4_total_hit_length( X.S.oa, lisSize, V.k ) ;
-				if ( hitLen < hitLenRequired || t4_total_hit_length( X.S.ob, lisSize, V.k ) < hitLenRequired )
-				{
-					s = e ;
-					continue ;
-				}
-				if ( n >= X.ovlCap || X.hcUsed + lisSize > X.hcCap )
-				{
-					X.overflow = 1 ;
-					return n ;
-				}
-				T4ROvl &no = X.ovl[n] ;
-				no.seqIdx = (int)( ( keys[i] >> T4_KEY_IDX_SHIFT ) & ( ( 1u << T4_KEY_IDX_BITS ) - 1 ) ) ;
-				no.readStart = X.S.oa[0] ;
-				no.readEnd = X.S.oa[lisSize - 1] + V.k - 1 ;
-				no.strand = ( keys[i] >> T4_KEY_STRAND_SHIFT ) ? 1 : -1 ;
-				no.seqStart = X.S.ob[0] ;
-				no.seqEnd = X.S.ob[lisSize - 1] + V.k - 1 ;
-				no.matchCnt = 2 * hitLen ;
-				no.indelCnt = 0 ;
-				no.similarity = 0 ;
-				no.hcStart = X.hcUsed ;
-				no.hcCnt = lisSize ;
-				no.infoFromHits = 0 ;
-				for ( int x = 0 ; x < lisSize ; ++x )
-				{
-					X.hcA[X.hcUsed + x] = X.S.oa[x] ;
-					X.hcB[X.hcUsed + x] = X.S.ob[x] ;
-				}
-				X.hcUsed += lisSize ;
-				++n ;
-				s = e ;
+				X.hcA[X.hcUsed + x] = X.S.oa[x] ;
+				X.hcB[X.hcUsed + x] = X.S.ob[x] ;
 			}
-		}
+			X.hcUsed += lisSize ;
+			++n ;
+			return true ;
+		} ) ;
+		if ( !walked ) // X.overflow
+			return n ;
 		i = j ;
 	}
 	return n ;
@@ -209,9 +163,9 @@ T4_HD inline int t4_ref_vj_overlaps( const u64 *keys, int H, const T4RefView &V,
 	int nv = 0 ;
 	for ( int i = 0 ; i < H ; ++i )
 	{
-		const int idx = (int)( ( keys[i] >> T4_KEY_IDX_SHIFT ) & ( ( 1u << T4_KEY_IDX_BITS ) - 1 ) ) ;
+		const int idx = t4_key_idx( keys[i] ) ;
 		const char c3 = V.name( idx )[3] ;
-		const int b = t4_rk_b( keys[i] ) ;
+		const int b = t4_key_b( keys[i] ) ;
 		if ( ( c3 == 'V' && b >= V.len( idx ) - 31 ) || ( c3 == 'J' && b < 31 ) )
 			X.vj[nv++] = keys[i] ; // a subsequence of a sorted array: still sorted
 	}
@@ -240,7 +194,7 @@ T4_HD inline int t4_ref_vj_overlaps( const u64 *keys, int H, const T4RefView &V,
 		}
 	if ( maxMatchCnt == 0 )
 		return 0 ;
-	const T4ROvl a = X.ovl[tagi], b = X.ovl[tagj] ;
+	const T4Ovl a = X.ovl[tagi], b = X.ovl[tagj] ;
 	X.ovl[0] = a ;
 	X.ovl[1] = b ;
 	return 2 ;
@@ -373,63 +327,13 @@ T4_HD inline int t4_global_alignment( const char *t, int lent, const char *p, in
 	return ret ;
 }
 
-// struct _overlap::operator< (SeqSet.hpp:104): higher priority first
-T4_HD inline bool t4_rovl_less( const T4ROvl &a, const T4ROvl &b )
-{
-	if ( a.matchCnt != b.matchCnt )
-		return a.matchCnt > b.matchCnt ;
-	else if ( a.similarity != b.similarity )
-		return a.similarity > b.similarity ;
-	else if ( a.readEnd - a.readStart != b.readEnd - b.readStart )
-		return a.readEnd - a.readStart > b.readEnd - b.readStart ;
-	else if ( a.seqIdx != b.seqIdx )
-		return a.seqIdx < b.seqIdx ;
-	else if ( a.strand != b.strand )
-		return a.strand < b.strand ;
-	else if ( a.readStart != b.readStart )
-		return a.readStart < b.readStart ;
-	else if ( a.readEnd != b.readEnd )
-		return a.readEnd < b.readEnd ;
-	else if ( a.seqStart != b.seqStart )
-		return a.seqStart < b.seqStart ;
-	else
-		return a.seqEnd < b.seqEnd ;
-}
-
-T4_HD inline void t4_rovl_sort( T4ROvl *o, T4ROvl *tmp, int n ) // rank sort: the order is total on distinct overlaps
+// std::sort( overlaps ), serial
+T4_HD inline void t4_ovl_sort( T4Ovl *o, T4Ovl *tmp, int n )
 {
 	for ( int i = 0 ; i < n ; ++i )
-	{
-		int rank = 0 ;
-		for ( int j = 0 ; j < n ; ++j )
-			if ( j != i && ( t4_rovl_less( o[j], o[i] ) || ( j < i && !t4_rovl_less( o[i], o[j] ) ) ) )
-				++rank ;
-		tmp[rank] = o[i] ;
-	}
+		tmp[t4_ovl_rank( o, n, i )] = o[i] ;
 	for ( int i = 0 ; i < n ; ++i )
 		o[i] = tmp[i] ;
-}
-
-// SeqSet::IsOverlapLowComplex (SeqSet.hpp:590-620)
-T4_HD inline bool t4_rovl_low_complex( const char *r, const T4ROvl &o )
-{
-	int cnt[4] = { 0, 0, 0, 0 } ;
-	for ( int i = o.readStart ; i <= o.readEnd ; ++i )
-	{
-		if ( r[i] == 'N' )
-			continue ;
-		++cnt[ t4_nuc( r[i] ) ] ;
-	}
-	int lowCnt = 0, lowTotalCnt = 0 ;
-	for ( int i = 0 ; i < 4 ; ++i )
-		if ( cnt[i] <= 2 )
-		{
-			++lowCnt ;
-			lowTotalCnt += cnt[i] ;
-		}
-	if ( lowTotalCnt * 7 >= o.readEnd - o.readStart + 1 )
-		return false ;
-	return lowCnt >= 2 ;
 }
 
 // SeqSet::GetOverlapsFromRead( read, 0, -1, readType 0, false ) on a reference set, from the sorted hits on: chains (or the
@@ -447,7 +351,7 @@ T4_HD inline int t4_ref_overlaps_from_read( const u64 *keys, int H, const char *
 		if ( overlapCnt == 0 || X.overflow )
 			return 0 ;
 	}
-	t4_rovl_sort( X.ovl, X.ovlTmp, overlapCnt ) ;
+	t4_ovl_sort( X.ovl, X.ovlTmp, overlapCnt ) ;
 	{
 		int kk = 1 ;
 		for ( int i = 1 ; i < overlapCnt ; ++i ) // readType 0: keep the strand of the best overlap (SeqSet.hpp:1601-1616)
@@ -463,7 +367,7 @@ T4_HD inline int t4_ref_overlaps_from_read( const u64 *keys, int H, const char *
 	const int k = V.k ;
 	for ( int i = 0 ; i < overlapCnt ; ++i )
 	{
-		T4ROvl &o = X.ovl[i] ;
+		T4Ovl &o = X.ovl[i] ;
 		const char *r = o.strand == 1 ? read : rc ;
 		const char *cons = V.cons( o.seqIdx ) ;
 		o.infoFromHits = i ;
@@ -543,7 +447,7 @@ T4_HD inline int t4_ref_overlaps_from_read( const u64 *keys, int H, const char *
 			o.similarity = (double)matchCnt / ( o.seqEnd - o.seqStart + 1 + o.readEnd - o.readStart + 1 ) ;
 		else
 			o.similarity = 0 ;
-		if ( t4_rovl_low_complex( r, o ) )
+		if ( t4_low_complex( r, o ) )
 			o.similarity = 0 ;
 	}
 	int kk = 0 ;
@@ -559,42 +463,6 @@ T4_HD inline int t4_ref_overlaps_from_read( const u64 *keys, int H, const char *
 }
 
 // ---- SeqSet::AnnotateRead( read, 0, geneOverlap, NULL, NULL ) (SeqSet.hpp:6016-6340, the detailLevel 0 statements) ----------
-// SeqSet::GetGeneType / GetChainType, SeqSet.hpp:5076-5100, 5132-5155
-T4_HD inline int t4_ref_chain_type( const char *name )
-{
-	if ( name[0] == 'I' )
-	{
-		if ( name[2] == 'H' ) return 0 ;
-		else if ( name[2] == 'K' ) return 1 ;
-		else if ( name[2] == 'L' ) return 2 ;
-	}
-	else if ( name[0] == 'T' )
-	{
-		if ( name[2] == 'A' ) return 3 ;
-		else if ( name[2] == 'B' ) return 4 ;
-		else if ( name[2] == 'G' ) return 5 ;
-		else if ( name[2] == 'D' ) return 6 ;
-	}
-	return 8 ;
-}
-
-T4_HD inline int t4_ref_gene_type( const char *name )
-{
-	if ( name[0] == 'N' && name[1] == 'o' )
-		return -1 ;
-	switch ( name[3] )
-	{
-		case 'V': return 0 ;
-		case 'D': return ( name[4] >= '0' && name[4] <= '9' ) ? 1 : 3 ;
-		case 'J': return 2 ;
-		case 'L':
-			if ( t4_ref_chain_type( name ) == 2 )
-				return -1 ; // IGLL genes
-			return 3 ;
-		default: return 3 ;
-	}
-}
-
 // SeqSet::GetContigIntervals (SeqSet.hpp:5289-5321): the read is cut where gapN = 7 N's fall into a window of 7
 T4_HD inline int t4_contig_intervals( const char *read, int len, int *ca, int *cb, int cap )
 {
@@ -626,7 +494,7 @@ T4_HD inline int t4_contig_intervals( const char *read, int len, int *ca, int *c
 
 // From the overlaps of all contigs (read coordinates already shifted, each contig's list sorted) to geneOverlap[4]
 // (V, D, J, C): SeqSet.hpp:6230-6340 without the detailLevel >= 1 statements.  ovl is reordered in place.
-T4_HD inline int t4_annotate_select( T4ROvl *ovl, T4ROvl *tmp, int overlapCnt, int *seqUsed, int len, const T4RefView &V, T4ROvl geneOverlap[4] )
+T4_HD inline int t4_annotate_select( T4Ovl *ovl, T4Ovl *tmp, int overlapCnt, int *seqUsed, int len, const T4RefView &V, T4Ovl geneOverlap[4] )
 {
 	for ( int t = 0 ; t < 4 ; ++t )
 	{
@@ -638,16 +506,16 @@ T4_HD inline int t4_annotate_select( T4ROvl *ovl, T4ROvl *tmp, int overlapCnt, i
 		geneOverlap[t].similarity = 0 ;
 		geneOverlap[t].infoFromHits = 0 ;
 		geneOverlap[t].hcStart = geneOverlap[t].hcCnt = 0 ;
-		geneOverlap[t].pad = 0 ;
+		geneOverlap[t].preMatchCnt = 0 ;
 	}
-	t4_rovl_sort( ovl, tmp, overlapCnt ) ;
+	t4_ovl_sort( ovl, tmp, overlapCnt ) ;
 	for ( int i = 0 ; i < V.nSeqs ; ++i )
 		seqUsed[i] = -1 ;
 	const double geneSimilarity = 0.8 ;
 	int k = 0 ;
 	for ( int i = 0 ; i < overlapCnt ; ++i )
 	{
-		const int geneType = t4_ref_gene_type( V.name( ovl[i].seqIdx ) ) ;
+		const int geneType = t4_gene_type( V.name( ovl[i].seqIdx ), V.nameLen( ovl[i].seqIdx ) ) ;
 		if ( geneType < 0 || geneType == 1 )
 			continue ;
 		if ( seqUsed[ ovl[i].seqIdx ] == -1 && ovl[i].similarity >= geneSimilarity )
@@ -658,12 +526,12 @@ T4_HD inline int t4_annotate_select( T4ROvl *ovl, T4ROvl *tmp, int overlapCnt, i
 		}
 		else if ( seqUsed[ ovl[i].seqIdx ] != -1 && geneType == 2 )
 		{
-			T4ROvl &baseline = ovl[ seqUsed[ ovl[i].seqIdx ] ] ;
+			T4Ovl &baseline = ovl[ seqUsed[ ovl[i].seqIdx ] ] ;
 			if ( ovl[i].matchCnt == baseline.matchCnt && ovl[i].similarity == baseline.similarity )
 			{
 				int j ;
 				for ( j = 0 ; j < k ; ++j )
-					if ( t4_ref_gene_type( V.name( ovl[j].seqIdx ) ) == 3 )
+					if ( t4_gene_type( V.name( ovl[j].seqIdx ), V.nameLen( ovl[j].seqIdx ) ) == 3 )
 						break ;
 				if ( j < k && ovl[i].readEnd <= ovl[j].readStart + 3 )
 				{
@@ -687,7 +555,7 @@ T4_HD inline int t4_annotate_select( T4ROvl *ovl, T4ROvl *tmp, int overlapCnt, i
 		if ( chain && !( name[2] == chain || ( name[2] == 'D' && chain == 'A' ) || ( name[2] == 'A' && chain == 'D' ) ) )
 			continue ;
 		chain = name[2] ;
-		const int geneType = t4_ref_gene_type( name ) ;
+		const int geneType = t4_gene_type( name, V.nameLen( ovl[i].seqIdx ) ) ;
 		if ( geneType >= 0 && geneOverlap[geneType].seqIdx == -1 )
 			geneOverlap[geneType] = ovl[i] ;
 	}
@@ -726,34 +594,16 @@ T4_D inline void c_ref_get_overlaps( T4Ctx &cx, T4Op *op )
 	if ( op->len >= st->kmerLength )
 	{
 		ret = 0 ;
-		int anyBig = 0 ;
-		u32 H = c_get_hits( cx, op->len, 0, -1, false, &anyBig, true ) ;
-		if ( ( anyBig || (int)H > P->hMax ) && cx.tid == 0 )
-			t4_raise( cx, anyBig ? T4_E_UNSUPPORTED : T4_E_NOMEM, 7 ) ;
-		if ( !c_uniform_error( cx ) && H > 0 )
+		const u64 *sorted = 0 ;
+		bool failed ;
+		const u32 H = c_ref_sorted_hits( cx, op->len, P->hMax, 7, &sorted, failed ) ;
+		if ( H > 0 )
 		{
-			u64 *a = cx.P<u64>( st->keysAOff ) ;
-			u64 *b = cx.P<u64>( st->keysBOff ) ;
-			T4_PAR_FOR( i, H )
-			{
-				const u64 kx = a[i] ;
-				a[i] = ( kx & ( ~0ull << T4_KEY_IDX_SHIFT ) ) | ( (u64)t4_key_a( kx ) << 30 ) | ( (u64)t4_key_b( kx ) << 1 ) | ( kx & 1 ) ;
-			}
-			T4_SYNC() ;
-			const u64 *sorted = c_sort_keys( cx, a, b, H ) ;
 			if ( cx.tid == 0 )
 			{
 				T4AnnotScratch X ;
 				t4_annot_carve( X, t4_x<char>( P->scratch ), (int)H, st->nomatchGapLimit, op->len ) ;
-				T4RefView V ;
-				V.seqs = cx.P<T4Contig>( st->seqsOff ) ;
-				V.A = cx.A ;
-				V.nSeqs = st->nSeqs ;
-				V.k = st->kmerLength ;
-				V.radius = st->radius ;
-				V.hitLenRequired = st->hitLenRequired ;
-				V.nomatchGapLimit = st->nomatchGapLimit ;
-				V.refSeqSimilarity = 0.75 ; // SeqSet.hpp:2566
+				const T4RefView V = t4_ref_view( cx ) ;
 				int n = t4_ref_overlaps_from_read( sorted, (int)H, sm->read, sm->rc, op->len, V, X ) ;
 				if ( X.overflow )
 					t4_raise( cx, T4_E_NOMEM, 8 ) ;
@@ -761,7 +611,7 @@ T4_D inline void c_ref_get_overlaps( T4Ctx &cx, T4Op *op )
 				double *sim = (double *)( out + 8 * op->outCap ) ;
 				for ( int i = 0 ; i < n && i < op->outCap ; ++i )
 				{
-					const T4ROvl &o = X.ovl[i] ;
+					const T4Ovl &o = X.ovl[i] ;
 					out[8 * i] = o.seqIdx ; out[8 * i + 1] = o.readStart ; out[8 * i + 2] = o.readEnd ; out[8 * i + 3] = o.seqStart ;
 					out[8 * i + 4] = o.seqEnd ; out[8 * i + 5] = o.strand ; out[8 * i + 6] = o.matchCnt ; out[8 * i + 7] = o.indelCnt ;
 					sim[i] = o.similarity ;
@@ -792,30 +642,6 @@ struct T4AnnotParams
 	int pad ;
 } ;
 
-// hits of the read in sm->read / rc (length len) against the attached gene set, sorted in SortHits order.  Collective;
-// returns the hit count (keys in *sorted), sets failed on a device error.
-T4_D inline u32 c_ref_sorted_hits( T4Ctx &cx, int len, int hMax, const u64 **sorted, bool &failed )
-{
-	T4Stream *st = cx.st ;
-	int anyBig = 0 ;
-	u32 H = c_get_hits( cx, len, 0, -1, false, &anyBig, true ) ;
-	if ( ( anyBig || (int)H > hMax ) && cx.tid == 0 )
-		t4_raise( cx, anyBig ? T4_E_UNSUPPORTED : T4_E_NOMEM, 7 ) ;
-	failed = c_uniform_error( cx ) != 0 ;
-	if ( failed || H == 0 )
-		return 0 ;
-	u64 *a = cx.P<u64>( st->keysAOff ) ;
-	u64 *b = cx.P<u64>( st->keysBOff ) ;
-	T4_PAR_FOR( i, H )
-	{
-		const u64 kx = a[i] ;
-		a[i] = ( kx & ( ~0ull << T4_KEY_IDX_SHIFT ) ) | ( (u64)t4_key_a( kx ) << 30 ) | ( (u64)t4_key_b( kx ) << 1 ) | ( kx & 1 ) ;
-	}
-	T4_SYNC() ;
-	*sorted = c_sort_keys( cx, a, b, H ) ;
-	return H ;
-}
-
 T4_D inline void c_ref_annotate( T4Ctx &cx, T4Op *op )
 {
 	const T4AnnotParams *P = t4_x<T4AnnotParams>( op->out ) ;
@@ -829,15 +655,7 @@ T4_D inline void c_ref_annotate( T4Ctx &cx, T4Op *op )
 	u64 *cursor = t4_x<u64>( P->cursor ) ;
 	char *scratch = t4_x<char>( P->scratch ) + (u64)op->n * P->scratchStride ;
 	c_assign_attach( cx, cx.P<T4Stream>( P->setOff ) ) ;
-	T4RefView V ;
-	V.seqs = cx.P<T4Contig>( st->seqsOff ) ;
-	V.A = cx.A ;
-	V.nSeqs = st->nSeqs ;
-	V.k = st->kmerLength ;
-	V.radius = st->radius ;
-	V.hitLenRequired = st->hitLenRequired ;
-	V.nomatchGapLimit = st->nomatchGapLimit ;
-	V.refSeqSimilarity = 0.75 ;
+	const T4RefView V = t4_ref_view( cx ) ;
 	bool failed = false ;
 	while ( !failed )
 	{
@@ -880,7 +698,7 @@ T4_D inline void c_ref_annotate( T4Ctx &cx, T4Op *op )
 				continue ; // GetOverlapsFromRead returns -1: no overlaps
 			c_load_read( cx, src + ca, clen ) ;
 			const u64 *sorted = 0 ;
-			const u32 H = c_ref_sorted_hits( cx, clen, P->hMax, &sorted, failed ) ;
+			const u32 H = c_ref_sorted_hits( cx, clen, P->hMax, 7, &sorted, failed ) ;
 			if ( failed )
 				break ;
 			if ( H > 0 && cx.tid == 0 )
@@ -896,7 +714,7 @@ T4_D inline void c_ref_annotate( T4Ctx &cx, T4Op *op )
 						X.ovl[i].readStart += ca ;
 						X.ovl[i].readEnd += ca ;
 					}
-					t4_rovl_sort( X.ovl, X.ovlTmp, n ) ;
+					t4_ovl_sort( X.ovl, X.ovlTmp, n ) ;
 					for ( int i = 0 ; i < n ; ++i )
 						X.acc[nAcc + i] = X.ovl[i] ;
 					nAcc += n ;
@@ -908,7 +726,7 @@ T4_D inline void c_ref_annotate( T4Ctx &cx, T4Op *op )
 			break ;
 		if ( cx.tid == 0 )
 		{
-			T4ROvl go[4] ;
+			T4Ovl go[4] ;
 			t4_annotate_select( X.acc, X.ovlTmp, nAcc, X.seqUsed, len, V, go ) ;
 			for ( int t = 0 ; t < 4 ; ++t )
 			{

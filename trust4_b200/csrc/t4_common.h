@@ -108,7 +108,7 @@ struct T4Ovl               // SeqSet.hpp:76 `_overlap`
 	int matchCnt ;
 	int indelCnt ;
 	double similarity ;
-	int hcStart, hcCnt ;   // hitCoords = keys[hcStart .. hcStart+hcCnt) of the sorted hit array
+	int hcStart, hcCnt ;   // hitCoords = keys[hcStart .. hcStart+hcCnt) of the sorted hit array (rough annotation: of its chain pool)
 	int preMatchCnt ;      // matchCnt before scoring (2*hitLen), consulted by the pre-filters SeqSet.hpp:1705-1794
 	int infoFromHits ;
 } ;

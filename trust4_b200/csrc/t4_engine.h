@@ -285,6 +285,17 @@ T4_HD inline int t4_key_c( u64 k ) { return (int)( ( k >> T4_KEY_C_SHIFT ) & T4_
 T4_HD inline int t4_key_a( u64 k ) { return t4_key_b( k ) + t4_key_c( k ) ; }
 T4_HD inline int t4_key_big( u64 k ) { return (int)( k & 1 ) ; }
 
+// The same hit re-keyed into SortHits order (strand, idx, a, b, repeats), SeqSet.hpp:1306: the read offset a takes bits
+// [40:30] in place of the diagonal, so sorted keys group by (strand, contig) and ascend in a, then b.  Strand, contig, b
+// and the repeats bit keep their places: read them with t4_key_strand / idx / b / big.  T4_KEY_INVALID stays invalid.
+T4_HD inline u64 t4_sortkey_of( u64 k )
+{
+	if ( k == T4_KEY_INVALID )
+		return k ;
+	return ( k & ( ~0ull << T4_KEY_IDX_SHIFT ) ) | ( (u64)t4_key_a( k ) << 30 ) | ( (u64)t4_key_b( k ) << T4_KEY_B_SHIFT ) | ( k & 1 ) ;
+}
+T4_HD inline int t4_sortkey_a( u64 k ) { return (int)( ( k >> 30 ) & 0x7ff ) ; }
+
 // ---------------------------------------------------------------------------
 // k-mer directory + postings (KmerIndex.hpp).  Open addressing, 32-byte slots.
 // ---------------------------------------------------------------------------
@@ -2253,7 +2264,22 @@ T4_HD inline bool t4_ovl_less( const T4Ovl &a, const T4Ovl &b )
 }
 
 // std::sort( overlaps ) with operator< (a strict total order on distinct overlaps, so any correct sort
-// yields the reference's sequence).  Rank sort: n is small (tens, rarely hundreds).
+// yields the reference's sequence) as a rank sort: n is small (tens, rarely hundreds).  The place of ovl[i]; equal
+// overlaps keep their order.
+T4_HD inline int t4_ovl_rank( const T4Ovl *ovl, int n, int i )
+{
+	const T4Ovl me = ovl[i] ;
+	int rank = 0 ;
+	for ( int j = 0 ; j < n ; ++j )
+	{
+		if ( j == i )
+			continue ;
+		if ( t4_ovl_less( ovl[j], me ) || ( j < i && !t4_ovl_less( me, ovl[j] ) ) )
+			++rank ;
+	}
+	return rank ;
+}
+
 T4_D inline void c_sort_overlaps( T4Ctx &cx, int n )
 {
 	if ( n <= 1 )
@@ -2261,18 +2287,7 @@ T4_D inline void c_sort_overlaps( T4Ctx &cx, int n )
 	T4Ovl *ovl = cx.P<T4Ovl>( cx.st->ovlOff ) ;
 	T4Ovl *tmp = cx.P<T4Ovl>( cx.st->ovlTmpOff ) ;
 	T4_PAR_FOR( i, n )
-	{
-		T4Ovl me = ovl[i] ;
-		int rank = 0 ;
-		for ( int j = 0 ; j < n ; ++j )
-		{
-			if ( j == i )
-				continue ;
-			if ( t4_ovl_less( ovl[j], me ) || ( j < i && !t4_ovl_less( me, ovl[j] ) ) )
-				++rank ;
-		}
-		tmp[rank] = me ;
-	}
+		tmp[t4_ovl_rank( ovl, n, i )] = ovl[i] ;
 	T4_SYNC() ;
 	T4_PAR_FOR( i, n )
 		ovl[i] = tmp[i] ;
@@ -2280,7 +2295,7 @@ T4_D inline void c_sort_overlaps( T4Ctx &cx, int n )
 }
 
 // SeqSet::IsOverlapLowComplex (SeqSet.hpp:590)
-T4_D inline bool t4_low_complex( const char *r, const T4Ovl &o )
+T4_HD inline bool t4_low_complex( const char *r, const T4Ovl &o )
 {
 	int cnt[4] = {0, 0, 0, 0} ;
 	for ( int i = o.readStart ; i <= o.readEnd ; ++i )
@@ -3082,7 +3097,7 @@ T4_D inline void c_score_all_warp( T4Ctx &cx, T4Ovl *ovl, int overlapCnt, const 
 // gene names
 // ---------------------------------------------------------------------------
 // SeqSet::GetChainType (SeqSet.hpp:5132)
-T4_D inline int t4_chain_type( const char *name )
+T4_HD inline int t4_chain_type( const char *name )
 {
 	if ( name[0] == 'I' )
 	{
@@ -3101,7 +3116,7 @@ T4_D inline int t4_chain_type( const char *name )
 }
 
 // SeqSet::GetGeneType (SeqSet.hpp:5076) on name[0..n)
-T4_D inline int t4_gene_type( const char *name, int n )
+T4_HD inline int t4_gene_type( const char *name, int n )
 {
 	// the reference reads name[3], name[4] of a NUL-terminated string; positions past the end read as '\0'
 	char c0 = n > 0 ? name[0] : 0, c1 = n > 1 ? name[1] : 0, c3 = n > 3 ? name[3] : 0, c4 = n > 4 ? name[4] : 0 ;
@@ -3116,7 +3131,7 @@ T4_D inline int t4_gene_type( const char *name, int n )
 		{
 			char tmp[3] = { c0, c1, n > 2 ? name[2] : (char)0 } ;
 			if ( t4_chain_type( tmp ) == 2 )
-				return -1 ;
+				return -1 ; // IGLL genes
 			return 3 ;
 		}
 		default: return 3 ;
@@ -5338,17 +5353,11 @@ T4_D inline void c_run_op( T4Ctx &cx, T4Op *op, const int *gapLimitTable )
 				u32 H = c_get_hits( cx, op->len, op->strand, op->barcode, op->repetitive != 0, &anyBig ) ;
 				u64 *a = cx.P<u64>( st->keysAOff ) ;
 				u64 *b = cx.P<u64>( st->keysBOff ) ;
-				// re-key to SortHits order: (strand, idx, a, b)
 				const T4Pos *pos = cx.P<T4Pos>( st->posOff ) ;
 				const int m = op->len - st->kmerLength + 1 ;
 				T4_PAR_FOR( i, H )
-				{
-					u64 kx = a[i] ;
-					if ( kx == T4_KEY_INVALID )
-						continue ;
-					u64 aa = (u64)t4_key_a( kx ) ;
-					a[i] = ( kx & ( ~0ull << T4_KEY_IDX_SHIFT ) ) | ( aa << 30 ) | ( (u64)t4_key_b( kx ) << 1 ) | ( kx & 1 ) ;
-				}
+					if ( a[i] != T4_KEY_INVALID ) // no store for the hits the barcode filter dropped
+						a[i] = t4_sortkey_of( a[i] ) ;
 				T4_SYNC() ;
 				u64 *sorted = c_sort_keys( cx, a, b, H ) ;
 				int32_t *out = t4_x<int32_t>( op->out ) ;
@@ -5358,8 +5367,8 @@ T4_D inline void c_run_op( T4Ctx &cx, T4Op *op, const int *gapLimitTable )
 					if ( kx == T4_KEY_INVALID || i >= op->outCap )
 						continue ;
 					int strand = t4_key_strand( kx ) ;
-					int aa = (int)( ( kx >> 30 ) & 0x7ff ) ;
-					int bb = (int)( ( kx >> 1 ) & T4_KEY_B_MASK ) ;
+					int aa = t4_sortkey_a( kx ) ;
+					int bb = t4_key_b( kx ) ;
 					out[5 * i] = t4_key_idx( kx ) ;
 					out[5 * i + 1] = bb ;
 					out[5 * i + 2] = aa ;

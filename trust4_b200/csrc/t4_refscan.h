@@ -11,8 +11,9 @@
 //
 // It is the volume scan of the pipeline (every raw read, typically 1e8) and read-only, so it runs like the AssignRead
 // pass: worker CTAs of the auxiliary kernel over the whole GPU, reads from an atomic cursor.  The probe and the key sort
-// are the engine's collectives; the bucket statistics and the chain logic are serial per read (a few hundred hits) and
-// plain C, identical on the device and in the test emulation.
+// are the engine's collectives (c_ref_sorted_hits); the bucket statistics and the chain walk (t4_ref_bucket_chains) are
+// serial per read (a few hundred hits) and plain C, identical on the device and in the test emulation.  The rough
+// annotation (t4_annot.h) calls both for every bucket.
 #ifndef T4_REFSCAN_H
 #define T4_REFSCAN_H
 
@@ -273,16 +274,19 @@ struct T4ScanScratch       // serial work arrays of one worker, each with room f
 
 // SeqSet::GetOverlapsFromHits( bucket, hitLenRequired, filter = 1, conservativeChain = false ) for ONE bucket of hits on a
 // reference sequence (SeqSet.hpp:763-1063, the isRef branch; every posting list of a reference set is far below the 10000
-// entries of the `repeats` rules, the caller checks).  keys[0..n): the bucket's hits, re-keyed (a in bits 30.., b in bits
-// 1..).  Returns matchCnt of the first overlap the reference would produce, or -1 when it produces none.
-T4_HD inline int t4_ref_bucket_overlap( const u64 *keys, int n, int k, int radius, int hitLenRequired, T4ScanScratch &S )
+// entries of the `repeats` rules, the caller checks).  keys[0..n): the bucket's hits in SortHits order (t4_sortkey_of).
+// For each chain that becomes an overlap, in the reference's order, calls emit( lisSize, hitLen ) with the chain in
+// S.oa / S.ob [0..lisSize) (read / gene offsets); the walk goes on while emit returns true.  Returns false when emit
+// stopped it.
+template <class Emit>
+T4_HD inline bool t4_ref_bucket_chains( const u64 *keys, int n, int k, int radius, int hitLenRequired, T4ScanScratch &S, Emit emit )
 {
 	const int minHitRequired = 3 ; // refMinHitRequired, SeqSet.hpp:778, 835-836
 	if ( n < minHitRequired )
-		return -1 ;
+		return true ;
 	for ( int i = 0 ; i < n ; ++i )
 	{
-		const int a = (int)( ( keys[i] >> 30 ) & 0x7ff ), b = (int)( ( keys[i] >> 1 ) & T4_KEY_B_MASK ) ;
+		const int a = t4_sortkey_a( keys[i] ), b = t4_key_b( keys[i] ) ;
 		S.w[i] = ( (u64)( a - b + T4_KEY_C_BIAS ) << 40 ) | ( (u64)b << 20 ) | (u64)a ; // CompSortHitCoordDiff: c, then b, then a
 	}
 	t4_heapsort64( S.w, n ) ;
@@ -321,14 +325,11 @@ T4_HD inline int t4_ref_bucket_overlap( const u64 *keys, int n, int k, int radiu
 			continue ;
 		}
 		const int hitLen = t4_total_hit_length( S.oa, lisSize, k ) ;
-		if ( hitLen < hitLenRequired || t4_total_hit_length( S.ob, lisSize, k ) < hitLenRequired )
-		{
-			s = e ;
-			continue ;
-		}
-		return 2 * hitLen ; // no.matchCnt, SeqSet.hpp:1037
+		if ( hitLen >= hitLenRequired && t4_total_hit_length( S.ob, lisSize, k ) >= hitLenRequired && !emit( lisSize, hitLen ) )
+			return false ;
+		s = e ;
 	}
-	return -1 ;
+	return true ;
 }
 
 // The decision of HasHitInSet( read, 0 ) from the read's hits sorted by (strand, gene, read offset, gene offset).
@@ -340,7 +341,7 @@ T4_HD inline int t4_has_hit_decide( const u64 *keys, int H, int k, int radius, i
 		const u64 g = keys[i] >> T4_KEY_IDX_SHIFT ; // strand | gene
 		int j = i + 1, readHitCount = 1 ;
 		for ( ; j < H && ( keys[j] >> T4_KEY_IDX_SHIFT ) == g ; ++j )
-			if ( ( ( keys[j] >> 30 ) & 0x7ff ) != ( ( keys[j - 1] >> 30 ) & 0x7ff ) )
+			if ( t4_sortkey_a( keys[j] ) != t4_sortkey_a( keys[j - 1] ) )
 				++readHitCount ;
 		const int tag = ( keys[i] >> T4_KEY_STRAND_SHIFT ) ? 1 : 0 ;
 		if ( readHitCount > max[tag] ) // genes in ascending order: the first of equals stays (SeqSet.hpp:3184-3188)
@@ -351,12 +352,21 @@ T4_HD inline int t4_has_hit_decide( const u64 *keys, int H, int k, int radius, i
 		}
 		i = j ;
 	}
+	// matchCnt of the first overlap GetOverlapsFromHits makes of a strand's bucket (SeqSet.hpp:1037), -1 when it makes none
+	auto firstMatchCnt = [&]( int tag ) {
+		int matchCnt = -1 ;
+		t4_ref_bucket_chains( keys + start[tag], size[tag], k, radius, hitLenRequired, S, [&]( int, int hitLen ) {
+			matchCnt = 2 * hitLen ;
+			return false ;
+		} ) ;
+		return matchCnt ;
+	} ;
 	int maxTag, found ;
 	if ( max[0] + k - 1 >= hitLenRequired && max[1] + k - 1 >= hitLenRequired )
 	{
 		// both strands look good: the better chain decides (SeqSet.hpp:3264-3301)
-		const int m0 = t4_ref_bucket_overlap( keys + start[0], size[0], k, radius, hitLenRequired, S ) ;
-		const int m1 = t4_ref_bucket_overlap( keys + start[1], size[1], k, radius, hitLenRequired, S ) ;
+		const int m0 = firstMatchCnt( 0 ) ;
+		const int m1 = firstMatchCnt( 1 ) ;
 		if ( m0 >= 0 && m1 >= 0 )
 			maxTag = m0 >= m1 ? 0 : 1 ;
 		else if ( m0 >= 0 )
@@ -368,7 +378,7 @@ T4_HD inline int t4_has_hit_decide( const u64 *keys, int H, int k, int radius, i
 	else
 	{
 		maxTag = max[1] >= max[0] ? 1 : 0 ;
-		found = t4_ref_bucket_overlap( keys + start[maxTag], size[maxTag], k, radius, hitLenRequired, S ) >= 0 ;
+		found = firstMatchCnt( maxTag ) >= 0 ;
 	}
 	if ( !found )
 		return 0 ;
@@ -394,6 +404,28 @@ T4_HD inline int t4_low_complexity_read( const char *seq, int len )
 		if ( cnt[x] <= 2 )
 			++lowCnt ;
 	return lowCnt >= 2 ? 1 : 0 ;
+}
+
+// Hits of the read in sm->read / rc (length len) against the attached gene set, sorted in SortHits order.  Collective;
+// returns the hit count (keys in *sorted).  A k-mer with > 10000 postings (not a reference gene set) raises
+// T4_E_UNSUPPORTED, more than hMax hits T4_E_NOMEM, both with `aux`; failed is set on any device error.
+T4_D inline u32 c_ref_sorted_hits( T4Ctx &cx, int len, int hMax, int aux, const u64 **sorted, bool &failed )
+{
+	T4Stream *st = cx.st ;
+	int anyBig = 0 ;
+	u32 H = c_get_hits( cx, len, 0, -1, false, &anyBig, true ) ;
+	if ( ( anyBig || (int)H > hMax ) && cx.tid == 0 )
+		t4_raise( cx, anyBig ? T4_E_UNSUPPORTED : T4_E_NOMEM, aux ) ;
+	failed = c_uniform_error( cx ) != 0 ;
+	if ( failed || H == 0 )
+		return 0 ;
+	u64 *a = cx.P<u64>( st->keysAOff ) ;
+	u64 *b = cx.P<u64>( st->keysBOff ) ;
+	T4_PAR_FOR( i, H )
+		a[i] = t4_sortkey_of( a[i] ) ;
+	T4_SYNC() ;
+	*sorted = c_sort_keys( cx, a, b, H ) ;
+	return H ;
 }
 
 // ---- T4_OP_REF_SCAN: worker loop -------------------------------------------------------------------------------------
@@ -439,26 +471,15 @@ T4_D inline void c_ref_scan( T4Ctx &cx, T4Op *op )
 			int result = 0 ;
 			if ( len >= st->kmerLength )
 			{
-				int anyBig = 0 ;
-				u32 H = c_get_hits( cx, len, 0, -1, false, &anyBig, true ) ;
-				if ( anyBig && cx.tid == 0 )
-					t4_raise( cx, T4_E_UNSUPPORTED, 6 ) ; // a k-mer with > 10000 postings: not a reference gene set
-				failed = c_uniform_error( cx ) != 0 ;
+				// SortHits order (strand, gene, read offset, gene offset): buckets become ranges.  No cap: the buffers grow
+				const u64 *sorted = 0 ;
+				const u32 H = c_ref_sorted_hits( cx, len, INT32_MAX, 6, &sorted, failed ) ;
 				if ( failed )
 					break ;
 				if ( H > 0 )
 				{
-					// SortHits order (strand, gene, read offset, gene offset): buckets become ranges
 					u64 *a = cx.P<u64>( st->keysAOff ) ;
-					u64 *b = cx.P<u64>( st->keysBOff ) ;
-					T4_PAR_FOR( i, H )
-					{
-						const u64 kx = a[i] ;
-						a[i] = ( kx & ( ~0ull << T4_KEY_IDX_SHIFT ) ) | ( (u64)t4_key_a( kx ) << 30 ) | ( (u64)t4_key_b( kx ) << 1 ) | ( kx & 1 ) ;
-					}
-					T4_SYNC() ;
-					u64 *sorted = c_sort_keys( cx, a, b, H ) ;
-					u64 *tmp = ( sorted == a ) ? b : a ;
+					u64 *tmp = ( sorted == a ) ? cx.P<u64>( st->keysBOff ) : a ;
 					// serial work arrays: 2 H packed words in the free key buffer (grown with the hit buffers: hitCap >= H, and
 					// the bucket and its window never exceed H together only when split -- so a second area holds the window)
 					T4_SYNC() ;
