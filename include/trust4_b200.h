@@ -284,6 +284,11 @@ int64_t t4_test_check_eq_bytes(t4_seqset *s, int64_t *bad);
 #define T4_N_COUNTERS 24
 int t4_last_counters(uint64_t *counters /* T4_N_COUNTERS */);
 
+/* CTAs of the stream kernel its registers are bounded for per SM (*target), and how many of them are resident per SM
+ * at the launch t4_streams_run uses: the current block size and the hit tile in dynamic shared memory (*resident,
+ * cudaOccupancyMaxActiveBlocksPerMultiprocessor; 0 in the emulation). */
+int t4_stream_residency(int *target, int *resident);
+
 /* ---- batch k-mer probe over frozen sets (the north-star "k-mer probe kernel") ----------------------------
  * SeqSet::GetHitsFromRead (SeqSet.hpp:1341-1501) + KmerIndex::Search (KmerIndex.hpp:104) for every record of an uploaded
  * workload against the set of its stream (record i belongs to set j iff desc_off[j] <= i < desc_off[j+1]; desc_off[0]

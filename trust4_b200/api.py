@@ -30,7 +30,7 @@ EXPORTS = [
     "seqset_output", "seqset_output_mem", "free", "seqset_get_contig", "has_motif",
     "reverse_complement_in_place", "seqset_get_hits", "seqset_get_overlaps", "dp_pos_weight_batch", "dp_hot_path_batch",
     "seqset_add_reads_batch", "streams_run", "workload_upload", "workload_free",
-    "streams_run_resident", "workload_results", "workload_events", "shard_reads", "last_counters", "streams_error",
+    "streams_run_resident", "workload_results", "workload_events", "shard_reads", "last_counters", "stream_residency", "streams_error",
     "hits_create", "hits_free", "streams_get_hits", "hits_stats", "hits_fetch", "hits_device_buffers",
     "seqset_index_checksum", "streams_pack_contigs", "streams_cycles",
     "seqset_release_finished_barcode", "seqset_release_shallow_contigs", "seqset_input_novel_fa", "seqset_contig_flags",
@@ -104,6 +104,7 @@ class Lib:
         f("workload_events", ci, [vp, vp])
         f("shard_reads", ci, [vp, C.c_int64, ci, ci, vp, vp])
         f("last_counters", ci, [vp])
+        f("stream_residency", ci, [C.POINTER(ci), C.POINTER(ci)])
         f("hits_create", vp, [C.c_int64, C.c_size_t])
         f("hits_free", None, [vp])
         f("streams_get_hits", ci, [C.POINTER(vp), ci, vp, vp, ci, vp, vp])

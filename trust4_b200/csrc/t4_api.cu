@@ -42,7 +42,8 @@
 static std::string g_err ;
 static void set_err( const std::string &s ) { g_err = s ; }
 
-#define T4_MIN_BLOCKS 4 // resident CTAs per SM the op kernels are register-bounded for
+#define T4_MIN_BLOCKS 4 // resident CTAs per SM the auxiliary and annotation kernels are register-bounded for
+#define T4_STREAM_BLOCKS 4 // ... and the stream kernel: 5 or 6 were measured slower per step (DESIGN.md §2a, §4)
 
 #if T4_CUDA
 #define CK( call )                                                                 \
@@ -57,7 +58,7 @@ static void set_err( const std::string &s ) { g_err = s ; }
 	} while ( 0 )
 
 // The kernels are thin wrappers: their bodies are device functions the emulation runs too (see the launchers below).
-__global__ void __launch_bounds__( T4_MAX_NT, T4_MIN_BLOCKS ) t4_stream_kernel( char *A, T4Op *ops, const int *gapTable )
+__global__ void __launch_bounds__( T4_MAX_NT, T4_STREAM_BLOCKS ) t4_stream_kernel( char *A, T4Op *ops, const int *gapTable )
 {
 	__shared__ T4Smem sm ;
 	T4Ctx cx = t4_ctx( A, ops[blockIdx.x].streamOff, &sm, threadIdx.x, blockDim.x ) ;
@@ -689,6 +690,21 @@ int T4_API( last_counters )( uint64_t *c )
 	int r = d2h( &g, E.A, sizeof( g ) ) ;
 	if ( r ) return r ;
 	memcpy( c, g.counters, sizeof( g.counters ) ) ;
+	return 0 ;
+}
+
+int T4_API( stream_residency )( int *target, int *resident )
+{
+	if ( !target || !resident )
+		return T4_E_INVAL ;
+	int r = ensure_up() ;
+	if ( r ) return r ;
+	*target = T4_STREAM_BLOCKS ;
+	*resident = 0 ; // the emulation runs one stream at a time
+#if T4_CUDA
+	// the launch of launch_ops(): E.nt threads and the hit tile as dynamic shared memory
+	CK( cudaOccupancyMaxActiveBlocksPerMultiprocessor( resident, t4_stream_kernel, E.nt, T4_HIT_TILE_BYTES ) ) ;
+#endif
 	return 0 ;
 }
 

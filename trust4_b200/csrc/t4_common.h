@@ -29,8 +29,14 @@ typedef int64_t i64;
 #else
 #define T4_BIG __noinline__
 #endif
+// The stream kernel's rarely taken paths (merge commits, novel contigs, k changes, consensus updates, purges, the rescue
+// pass, the per-call ops, the decision's on-demand ExtendOverlap) stay out of line even under T4_INLINE_ALL: their
+// register needs and spills then sit behind a call that runs rarely, not in the per-read phases of the driver loop,
+// which fit the kernel's register budget (T4_STREAM_BLOCKS) with far fewer spills (DESIGN.md §4).
+#define T4_RARE __noinline__
 #else
 #define T4_BIG inline
+#define T4_RARE inline
 #define T4_CUDA 0
 #define T4_HD
 #define T4_D

@@ -3274,7 +3274,7 @@ T4_D inline void s_update_consensus( T4Ctx &cx, int seqIdx, bool updateIndex )
 
 // SeqSet::UpdateAllConsensus (SeqSet.hpp:4525).  Collective: contigs are scanned in parallel, the rare
 // contigs that change are fixed up serially in slot order.
-T4_D T4_BIG void c_update_all_consensus( T4Ctx &cx )
+T4_D T4_RARE void c_update_all_consensus( T4Ctx &cx )
 {
 	T4Stream *st = cx.st ;
 	T4_SYNC() ;
@@ -3382,7 +3382,7 @@ T4_D inline int s_contig_shallow( T4Ctx &cx, int idx, int minCov )
 // ReleaseSeq), the others leave the index, get a final UpdateConsensus( i, false ) and, when their coverage is flat,
 // numRead = that coverage.  The reference then compresses / frees posWeight -- storage only: Output prints the same
 // numbers either way (SeqSet.hpp:10956-10992), so the columns stay as they are here.
-T4_D T4_BIG void c_release_barcode( T4Ctx &cx, int barcode, int contigMinCov )
+T4_D T4_RARE void c_release_barcode( T4Ctx &cx, int barcode, int contigMinCov )
 {
 	T4Stream *st = cx.st ;
 	T4Smem *sm = cx.sm ;
@@ -3449,7 +3449,7 @@ T4_D T4_BIG void c_release_barcode( T4Ctx &cx, int barcode, int contigMinCov )
 
 // SeqSet::ReleaseShallowContigs (SeqSet.hpp:10928): ReleaseSeq on every shallow contig; like the reference it leaves
 // their index entries behind (the driver calls it after the last AddRead, main.cpp:1952-1955).
-T4_D inline void c_release_shallow( T4Ctx &cx, int minCov )
+T4_D T4_RARE void c_release_shallow( T4Ctx &cx, int minCov )
 {
 	T4Stream *st = cx.st ;
 	T4_SYNC() ;
@@ -3491,7 +3491,7 @@ T4_D inline u32 t4_bc_slot( const T4BcTable &t, int barcode, bool claim )
 
 // SeqSet::Clean(false) + ChangeKmerLength (SeqSet.hpp:4591-4629): compact the slots, rebuild the index.
 // nomatchGapLimit is computed on the host (pow/log) and passed in.
-T4_D T4_BIG void c_change_kmer_length( T4Ctx &cx, int kl, int nomatchGapLimit )
+T4_D T4_RARE void c_change_kmer_length( T4Ctx &cx, int kl, int nomatchGapLimit )
 {
 	T4Stream *st = cx.st ;
 	T4_SYNC() ;
@@ -3538,7 +3538,7 @@ T4_D inline int t4_nomatch_gap_limit_table( int kl, const int *table )
 // ---------------------------------------------------------------------------
 // SeqSet::InputNovelRead (SeqSet.hpp:3028-3073).  Serial; reads cx.sm->read.
 // ---------------------------------------------------------------------------
-T4_D inline int c_input_novel_read( T4Ctx &cx, const char *id, int idLen, int len, int strand, int barcode )
+T4_D T4_RARE int c_input_novel_read( T4Ctx &cx, const char *id, int idLen, int len, int strand, int barcode )
 {
 	T4Stream *st = cx.st ;
 	T4Smem *sm = cx.sm ;
@@ -3665,7 +3665,7 @@ T4_D inline int c_dup_run_len( T4Ctx &cx, const t4_read_desc *descs, int i, int 
 }
 
 // exact ExtendOverlap of overlap i on demand (thread 0 of the decision loop)
-T4_D inline void s_make_exact( T4Ctx &cx, const char *r, int len, double factor, const T4Ovl *overlaps, T4Ovl *pre, int i )
+T4_D T4_RARE void s_make_exact( T4Ctx &cx, const char *r, int len, double factor, const T4Ovl *overlaps, T4Ovl *pre, int i )
 {
 #if T4_CUDA
 	long long t0 = clock64() ;
@@ -4286,7 +4286,7 @@ T4_D inline int s_decide_overlaps( T4Ctx &cx, const T4Ovl *overlaps, int overlap
 // of them and the read.  Rare (0.7 % of AddReads).  Thread 0.  Writes plan's kind, added, bail, ret, seqIdx and
 // readInConsensusOffset.  Borrows seqOffset (st->extOff, whose pre[] is dead after the decision) for the contigs'
 // positions in the merged contig.
-T4_D inline void s_merge_commit( T4Ctx &cx, T4Ovl *extendedOverlaps, int k, bool sortExtendedOverlaps, const char *r, int len,
+T4_D T4_RARE void s_merge_commit( T4Ctx &cx, T4Ovl *extendedOverlaps, int k, bool sortExtendedOverlaps, const char *r, int len,
 	int barcode, int *seqOffset, T4AddPlan &plan )
 {
 	int i, j ;
@@ -4881,6 +4881,35 @@ T4_D inline void s_mate_hint( const t4_read_desc *descs, int n, int i, int mateI
 	}
 }
 
+// main.cpp:1897-1940: AddRead again, at the rescue threshold, for every read whose first AddRead returned -2
+T4_D T4_RARE void c_rescue_pass( T4Ctx &cx, const t4_run_cfg &cfg, const t4_read_desc *descs, const int32_t *rescueList, int rescueCnt,
+	const u64 *packed, u64 packStride, const char *pool, int8_t *strands, int32_t *rescueRet, uint8_t *events )
+{
+	T4Stream *st = cx.st ;
+	for ( int x = 0 ; x < rescueCnt && !st->error ; ++x )
+	{
+		int i = rescueList[x] ;
+		const t4_read_desc d = descs[i] ;
+		if ( packed )
+			c_load_read_packed( cx, packed + (u64)i * packStride, d.len ) ;
+		else
+			c_load_read( cx, pool + d.seq_off, d.len ) ;
+		char name[2] = "" ;
+		int strand = 0 ;
+		int addRet = c_add_read( cx, d.len, name, strand, d.barcode, 1, cfg.repetitive != 0, t4_rescue_threshold( d.min_cnt ) ) ;
+		if ( cx.tid == 0 )
+		{
+			strands[i] = (int8_t)strand ;
+			rescueRet[i] = addRet ;
+			if ( events )
+				events[i] |= T4_EV_RESCUED ;
+		}
+		T4_SYNC() ;
+	}
+	if ( cfg.final_update && !st->error )
+		c_update_all_consensus( cx ) ;
+}
+
 T4_D inline void c_run_loop( T4Ctx &cx, T4Op *op, const int *gapLimitTable )
 {
 	T4Stream *st = cx.st ;
@@ -5148,30 +5177,7 @@ T4_D inline void c_run_loop( T4Ctx &cx, T4Op *op, const int *gapLimitTable )
 		c_update_all_consensus( cx ) ;
 	T4_PHASE( cx, 0 ) ;
 	if ( cfg.do_rescue && cfg.first_read_len <= 200 && !st->error )
-	{
-		for ( int x = 0 ; x < rescueCnt && !st->error ; ++x )
-		{
-			int i = rescueList[x] ;
-			const t4_read_desc d = descs[i] ;
-			if ( packed )
-				c_load_read_packed( cx, packed + (u64)i * packStride, d.len ) ;
-			else
-				c_load_read( cx, pool + d.seq_off, d.len ) ;
-			char name[2] = "" ;
-			int strand = 0 ;
-			int addRet = c_add_read( cx, d.len, name, strand, d.barcode, 1, cfg.repetitive != 0, t4_rescue_threshold( d.min_cnt ) ) ;
-			if ( cx.tid == 0 )
-			{
-				strands[i] = (int8_t)strand ;
-				rescueRet[i] = addRet ;
-				if ( events )
-					events[i] |= T4_EV_RESCUED ;
-			}
-			T4_SYNC() ;
-		}
-		if ( cfg.final_update && !st->error )
-			c_update_all_consensus( cx ) ;
-	}
+		c_rescue_pass( cx, cfg, descs, rescueList, rescueCnt, packed, packStride, pool, strands, rescueRet, events ) ;
 	if ( cx.tid == 0 )
 	{
 		st->assembledReadCnt = assembledReadCnt ;
@@ -5261,39 +5267,12 @@ T4_D inline void c_init_block( char *A, u64 base, const T4InitParams &ip, u32 b,
 	c_init_stream( cx, base + (u64)b * ip.footprint, ip ) ;
 }
 
-// ---------------------------------------------------------------------------
-// op dispatch: body of the stream kernel (one CTA = one T4Op)
-// ---------------------------------------------------------------------------
-T4_D inline void c_run_op( T4Ctx &cx, T4Op *op, const int *gapLimitTable )
+// the per-call ops of the C ABI (t4_seqset_add_read, ...): one op record each, never inside the driver loop
+T4_D T4_RARE void c_run_call_op( T4Ctx &cx, T4Op *op, const int *gapLimitTable )
 {
 	T4Stream *st = cx.st ;
-	T4Smem *sm = cx.sm ;
-	if ( st->error )
-	{
-		if ( cx.tid == 0 )
-			op->ret = st->error ;
-		return ;
-	}
-	if ( cx.tid == 0 )
-		for ( int i = 0 ; i < T4_N_COUNTERS ; ++i )
-			sm->ctr[i] = 0 ;
-#if T4_CUDA
-	if ( cx.tid == 0 )
-	{
-		for ( int i = 0 ; i < 8 ; ++i )
-			sm->ph[i] = 0 ;
-		sm->phCur = 0 ;
-		sm->phLast = clock64() ;
-	}
-#endif
-	T4_SYNC() ;
 	switch ( op->op )
 	{
-		case T4_OP_RUN_LOOP:
-			c_run_loop( cx, op, gapLimitTable ) ;
-			if ( cx.tid == 0 )
-				op->ret = st->error ? st->error : st->assembledReadCnt ;
-			break ;
 		case T4_OP_ADD_READ:
 		{
 			c_load_read( cx, t4_x<char>( op->read ), op->len ) ;
@@ -5421,6 +5400,42 @@ T4_D inline void c_run_op( T4Ctx &cx, T4Op *op, const int *gapLimitTable )
 		default:
 			break ;
 	}
+}
+
+// ---------------------------------------------------------------------------
+// op dispatch: body of the stream kernel (one CTA = one T4Op)
+// ---------------------------------------------------------------------------
+T4_D inline void c_run_op( T4Ctx &cx, T4Op *op, const int *gapLimitTable )
+{
+	T4Stream *st = cx.st ;
+	T4Smem *sm = cx.sm ;
+	if ( st->error )
+	{
+		if ( cx.tid == 0 )
+			op->ret = st->error ;
+		return ;
+	}
+	if ( cx.tid == 0 )
+		for ( int i = 0 ; i < T4_N_COUNTERS ; ++i )
+			sm->ctr[i] = 0 ;
+#if T4_CUDA
+	if ( cx.tid == 0 )
+	{
+		for ( int i = 0 ; i < 8 ; ++i )
+			sm->ph[i] = 0 ;
+		sm->phCur = 0 ;
+		sm->phLast = clock64() ;
+	}
+#endif
+	T4_SYNC() ;
+	if ( op->op == T4_OP_RUN_LOOP )
+	{
+		c_run_loop( cx, op, gapLimitTable ) ;
+		if ( cx.tid == 0 )
+			op->ret = st->error ? st->error : st->assembledReadCnt ;
+	}
+	else
+		c_run_call_op( cx, op, gapLimitTable ) ;
 	T4_SYNC() ;
 	if ( cx.tid == 0 && st->error && op->ret >= T4_E_BASE )
 		op->ret = st->error ;
